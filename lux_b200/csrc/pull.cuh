@@ -464,8 +464,9 @@ __global__ void __launch_bounds__(kFixBlock) pull_fixup_apply_kernel(const __gri
 // Block b scans its kFixBlock tiles, publishes its aggregate, looks back over the predecessors' published aggregates /
 // inclusive prefixes (the walk stops at the first aggregate that contains a completed vertex — almost always the
 // immediate predecessor), publishes its own inclusive prefix and applies.  Publication = value word first, then a
-// status word carrying the launch's epoch (no per-launch reset of the status array).  Deterministic: the combination
-// order is the tile order whatever the scheduling.
+// status word carrying the launch's epoch (no per-launch reset of the status array).  The combination follows tile
+// order, but its fp64 association depends on which prefixes were already published, so the last bit of a carry may
+// differ between runs (DESIGN §0); LUXB_FUSED_FIXUP=0 has a fixed association.
 template <class Prog>
 struct FixupChain {
   unsigned long long* value;   // [2 * n_blocks] aggregate / inclusive prefix values (Wide, bit-cast)

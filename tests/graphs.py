@@ -58,6 +58,52 @@ def two_components(n=2000):
     return O.edges_to_csc(n, s + d, d + s)
 
 
+def in_degrees(row_end):
+    return np.diff(np.concatenate([[0], row_end]).astype(np.int64))
+
+
+def mix32(ids, salt=0):
+    """A fixed 32-bit hash of vertex ids (splitmix64 finaliser, vectorised): spreads test values over the sources."""
+    z = np.asarray(ids).astype(np.uint64) + np.uint64(((salt + 1) * 0x9E3779B97F4A7C15) & (2**64 - 1))
+    z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+    z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+    return (z ^ (z >> np.uint64(31))) >> np.uint64(32)
+
+
+def exact_pr_inputs(nv, max_indeg, passes=4, salt=0):
+    """PageRank values on which every summation order is exact: integers cast to float32, so that one iteration from
+    them must equal the oracle's bit for bit whatever the sweep's reduction shape.
+
+    The largest raw sum S = sum of x[u] over a vertex's in-edges stays below 2^21: fp32 lane sums, shuffle scans and
+    partials of integers are then exact, and S off by one moves fma(0.15, S, init) by more than two ulps, which
+    survives the division by the out-degree.  Values x in {1..K}, K = floor(2^20 / max_indeg), make every edge count
+    and most misrouted sources visible in one pass.  Where K = 1 (a hub with more than 2^19 in-edges), `passes`
+    inputs: all ones (counts edges), then single hash bits of u in {0, 1} (finds misrouted sources).  `salt` picks
+    another set of values of the same kind."""
+    assert max_indeg < (1 << 21), "in-degree %d: sums of ones are no longer exact enough" % max_indeg
+    h = mix32(np.arange(nv, dtype=np.uint64), salt)
+    k = (1 << 20) // max(int(max_indeg), 1)
+    if k >= 2:
+        return [(np.uint64(1) + h % np.uint64(k)).astype(np.float32)]
+    return [np.ones(nv, np.float32)] + [((h >> np.uint64(b)) & np.uint64(1)).astype(np.float32) for b in range(passes - 1)]
+
+
+def exact_cf_inputs(users, items, max_item_indeg):
+    """Collaborative-filtering vectors on which every dot product, error, err * x_u and chunk sum is exact: users get
+    integers in {1, 2} on all 20 factors, items integers in {1..b} on factors 0-9 and zeros on factors 10-19.  Every
+    user -> item edge then has dot >= 10 > rating, so err < 0 and all terms of an item's accumulator have one sign:
+    its partial sums never exceed the final |acc|, which b keeps below 2^22 (|err * x_u| <= 2 * 20 b per edge).
+    For an item, factors 10-19 come out as rn(GAMMA * acc): bit-exact whether or not the update is contracted to an
+    FMA, and a function of the weight, the dot product and the source of every in-edge."""
+    b = int(min(8, max(1, (1 << 22) // (40 * max(int(max_item_indeg), 1)))))
+    x = np.zeros((users + items, 20), np.float32)
+    uid = np.arange(users, dtype=np.uint64)
+    x[:users] = (np.uint64(1) + ((mix32(uid, 1)[:, None] >> np.arange(20, dtype=np.uint64)) & np.uint64(1))).astype(np.float32)
+    iid = np.arange(items, dtype=np.uint64)
+    x[users:, :10] = (np.uint64(1) + (mix32(iid, 2)[:, None] >> (np.uint64(3) * np.arange(10, dtype=np.uint64))) % np.uint64(b)).astype(np.float32)
+    return x
+
+
 ALL_SMALL = {
     "hand5": hand5,
     "star": star,

@@ -1,8 +1,13 @@
-"""Executable model (numpy, CPU) of the pull kernel's cross-tile fix-up — the three-kernel segmented scan of
-lux_b200/csrc/pull.cuh (pull_fixup_scan / _blocks / _apply) — checked against the obvious sequential definition:
-carry into tile t = sum of the tail partials of the tiles since, and including, the last tile before t that completed
-a vertex.  Mirrors the CUDA control flow (256-tile blocks, 1024 serial chunks + shuffle scans) so that a change of the
-kernel's structure has a CPU-side regression check of the algebra, including n_blocks > 1024 (chunk length > 1)."""
+"""Executable models (numpy, CPU) of the pull sweeps' cross-tile fix-up in lux_b200/csrc/pull.cuh, checked against the
+obvious sequential definition: carry into tile t = sum of the tail partials of the tiles since, and including, the last
+tile before t that completed a vertex.
+  * the three-kernel segmented scan (pull_fixup_scan / _blocks / _apply, LUXB_FUSED_FIXUP=0): 256-tile blocks, 1024
+    serial chunks + shuffle scans, including n_blocks > 1024 (chunk length > 1);
+  * the fused chained scan (pull_fixup_fused_kernel, the default): in-block shuffle scan, then a decoupled look-back
+    over the predecessors' published aggregates / inclusive prefixes, with the publication state each predecessor may
+    be in when a block looks back (prefix published, or only the aggregate) and status words left by earlier launches.
+They mirror the CUDA control flow so that a change of the kernels' structure has a CPU-side regression check of the
+algebra.  Tails are integers: every summation order is exact, so the models must equal the definition bit for bit."""
 import numpy as np
 import pytest
 
@@ -80,3 +85,95 @@ def test_fixup_model_equals_sequential_definition(n, density):
     want = np.array(seq_scan_exclusive(flags, tails)[1])
     got = model_fixup(flags, tails)
     assert np.array_equal(got, want)
+
+
+def warp_scan_inclusive(f, v):
+    """Segmented inclusive scan over the last axis (32 lanes) with shfl_up steps, as the fix-up kernels run it."""
+    lane = np.arange(32)
+    for off in (1, 2, 4, 8, 16):
+        pf = np.zeros_like(f)
+        pv = np.zeros_like(v)
+        pf[..., off:], pv[..., off:] = f[..., :-off], v[..., :-off]
+        take = lane >= off  # seg_combine(sf, sv, pf, pv) on lanes >= off
+        v = np.where(take & (f == 0), pv + v, v)
+        f = np.where(take, f | pf, f)
+    return f, v
+
+
+def model_fused_fixup(flags, tails, rng, p_prefix, epoch=7, stop_after_one=False):
+    """pull_fixup_fused_kernel: returns the carry into every tile.  Blocks run in ticket order; when block b looks back,
+    each predecessor has published its aggregate and, with probability p_prefix, already its inclusive prefix.  A
+    prefix slot not yet written in this launch holds the status word and value an earlier launch left there.
+    stop_after_one: a deliberately wrong look-back that reads one predecessor only (the model's own sensitivity check)."""
+    n = len(flags)
+    nb = (n + FIX_BLOCK - 1) // FIX_BLOCK
+    F = np.zeros(nb * FIX_BLOCK, np.int64)
+    V = np.zeros(nb * FIX_BLOCK, np.float64)
+    F[:n], V[:n] = flags, tails
+    sf, sv = warp_scan_inclusive(F.reshape(nb, 8, 32), V.reshape(nb, 8, 32))
+    wf, wv = np.zeros((nb, 8), np.int64), np.zeros((nb, 8), np.float64)  # aggregate of the preceding warps
+    for w in range(1, 8):
+        a_f, a_v = sf[:, w - 1, 31], sv[:, w - 1, 31]
+        wv[:, w] = np.where(a_f == 0, wv[:, w - 1] + a_v, a_v)
+        wf[:, w] = a_f | wf[:, w - 1]
+    ef, ev = np.zeros_like(sf), np.zeros_like(sv)  # exclusive in-block prefix of each tile
+    ef[..., 1:], ev[..., 1:] = sf[..., :-1], sv[..., :-1]
+    ev = np.where(ef == 0, wv[..., None] + ev, ev)
+    ef = ef | wf[..., None]
+    af = sf[:, 7, 31] | wf[:, 7]  # block aggregates
+    av = np.where(sf[:, 7, 31] == 0, wv[:, 7] + sv[:, 7, 31], sv[:, 7, 31])
+    # chain slots: 2b = aggregate, 2b + 1 = inclusive prefix; status = (epoch << 2) | (flag << 1) | 1
+    value = rng.integers(-1000, 1000, 2 * nb).astype(np.float64)  # left by an earlier launch
+    status = ((epoch - 1) << 2) | (rng.integers(0, 2, 2 * nb) << 1) | 1
+    prefix_f, prefix_v, prefix_visible = np.zeros(nb, np.int64), np.zeros(nb), np.zeros(nb, bool)
+    bp_f, bp_v = np.zeros(nb, np.int64), np.zeros(nb)
+    for b in range(nb):
+        value[2 * b] = av[b]
+        status[2 * b] = (epoch << 2) | (int(af[b]) << 1) | 1
+        # what the predecessors have published by now: the real prefix, or still the stale slot of an earlier launch
+        for q in range(b):
+            if not prefix_visible[q] and rng.random() < p_prefix:
+                prefix_visible[q] = True
+                value[2 * q + 1] = prefix_v[q]
+                status[2 * q + 1] = (epoch << 2) | (int(prefix_f[q]) << 1) | 1
+        pf, pv = 0, 0.0
+        q = b - 1
+        while q >= 0 and not pf:
+            have_prefix = (status[2 * q + 1] >> 2) == epoch
+            s = status[2 * q + 1] if have_prefix else status[2 * q]
+            qf, qv = int((s >> 1) & 1), value[2 * q + (1 if have_prefix else 0)]
+            pv = pv if pf else qv + pv
+            pf |= qf
+            if have_prefix or stop_after_one:
+                break
+            q -= 1
+        bp_f[b], bp_v[b] = pf, pv
+        prefix_f[b] = int(af[b]) | pf
+        prefix_v[b] = av[b] if af[b] else pv + av[b]
+    carry = np.where(ef == 0, bp_v[:, None, None] + ev, ev)
+    return carry.reshape(-1)[:n]
+
+
+@pytest.mark.parametrize("n,density,p_prefix", [(1, 1.0, 0.5), (257, 0.01, 0.0), (5000, 0.0, 0.3), (5000, 0.02, 1.0),
+                                                (40000, 0.001, 0.5), (40000, 0.0005, 0.0), (60000, 0.3, 0.2)])
+def test_fused_fixup_model_equals_sequential_definition(n, density, p_prefix):
+    rng = np.random.default_rng(n + int(100 * p_prefix))
+    flags = (rng.random(n) < density).astype(np.int64)
+    tails = rng.integers(0, 100, n).astype(np.float64)
+    want = np.array(seq_scan_exclusive(flags, tails)[1])
+    got = model_fused_fixup(flags, tails, rng, p_prefix)
+    assert np.array_equal(got, want)
+
+
+def test_fused_fixup_model_sees_a_broken_look_back():
+    """The check is not vacuous: a look-back that stops after one predecessor's aggregate without a completed vertex
+    (instead of walking on to a published prefix or a flagged aggregate) drops the carry that crosses several blocks."""
+    n = 4 * FIX_BLOCK
+    flags = np.zeros(n, np.int64)
+    flags[10] = 1
+    tails = np.ones(n)
+    want = np.array(seq_scan_exclusive(flags, tails)[1])
+    assert np.array_equal(model_fused_fixup(flags, tails, np.random.default_rng(0), 0.0), want)
+    got = model_fused_fixup(flags, tails, np.random.default_rng(0), 0.0, stop_after_one=True)
+    assert not np.array_equal(got, want)
+    assert np.array_equal(got[:2 * FIX_BLOCK], want[:2 * FIX_BLOCK])

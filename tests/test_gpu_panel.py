@@ -4,7 +4,10 @@
     through L1, fp64 combine).  The split is normally enabled only on large partitions; LUXB_SB=1 with small blocks /
     thresholds forces it on small graphs so that every code path (many blocks, padding, hubs spanning pieces in both
     streams, (block, hub) pairs without edges, hubs whose edges all moved to the panel) is exercised;
-  * the merge-path tiles of pull.cuh (LUXB_SWEEP=merge), which CC / SSSP pull sweeps keep using."""
+  * the merge-path tiles of pull.cuh (LUXB_SWEEP=merge), which zero-copy graphs use.  CC / SSSP pull iterations run
+    the flagged sweep (and the split, where it is on) with their own vertex programs, like PageRank.
+The tolerance is wider than one wrong edge into a large hub; tests/test_gpu_exact.py compares the same paths bit for bit
+on inputs where every summation order is exact."""
 import numpy as np
 import pytest
 
