@@ -190,6 +190,8 @@ typedef struct {
   uint64_t panel_edges;      /* PageRank: local edges swept by the source-blocked (shared-memory) kernel; 0 = plain sweep */
   uint32_t panel_hubs;       /*   hub destinations of this partition */
   uint32_t panel_blocks;     /*   hot source blocks */
+  uint64_t cold_hub_edges;   /* PageRank, one rank: local (cold source -> hub) edges swept by segment of the cold values */
+  uint32_t cold_hub_segments; /*   cold source segments (0 = no cold-hub stream) */
 } luxb_stats_t;
 int luxb_stats(const luxb_graph* g, luxb_stats_t* out);
 /* Per-iteration trace of push apps (global active count, direction) for parity tests; returns #entries copied. */

@@ -18,7 +18,7 @@
 #include "runtime.cuh"
 
 using namespace luxb;
-static const char* const kPhaseName[12] = {"pull_tile", "fixup", "refresh", "rechunk", "barrier", "panel", "combine", "pack+push", "pull/bcast", "", "", ""};
+static const char* const kPhaseName[12] = {"pull_tile", "fixup", "refresh", "rechunk", "barrier", "panel", "combine", "pack+push", "pull/bcast", "cold_hub", "", ""};
 static void pt_mark(luxb_graph* g, int tag) {
   PhaseTimer& pt = g->pt;
   if (!pt.on) return;
@@ -33,7 +33,7 @@ static void pt_print(luxb_graph* g) {
     char line[1024];
     int n = snprintf(line, sizeof(line), "[luxb rank %d] phase means over %ld iterations:", g->cfg.rank, g->pt.cnt);
     double sum = 0;
-    for (int k = 0; k < 9; ++k) {
+    for (int k = 0; k < 10; ++k) {
       n += snprintf(line + n, sizeof(line) - n, " %s %.3f ms;", kPhaseName[k], g->pt.sum[k] / g->pt.cnt);
       sum += g->pt.sum[k] / g->pt.cnt;
     }
@@ -269,7 +269,7 @@ static int finish_layout(luxb_graph* g) {
   LUXB_TRY(dmalloc(&g->d_carry_flag, (uint64_t)g->n_tiles + 1));
   LUXB_TRY(dmalloc((uint64_t**)&g->d_block_agg, (uint64_t)g->n_fix_blocks + 1));
   LUXB_TRY(dmalloc(&g->d_block_flag, (uint64_t)g->n_fix_blocks + 1));
-  LUXB_TRY(dmalloc(&g->d_counters, 8));  // [0] edges scanned, [1] check mistakes, [2] pull tile counter, [3] big segments, [4] panel tile counter
+  LUXB_TRY(dmalloc(&g->d_counters, 8));  // [0] edges scanned, [1] check mistakes, [2] pull tile counter, [3] big segments, [4] panel / cold-hub tile counter
   LUXB_CUDA(cudaMemsetAsync(g->d_counters, 0, 8 * sizeof(unsigned long long), g->stream));
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
   return 0;
@@ -898,7 +898,10 @@ static int reset_label_state(luxb_graph* g, bool all_active) {
 }
 
 // Pin the hot copies in L2: persisting access-policy window on the hot buffer for every kernel of this stream,
-// everything else is treated as streaming when it misses.  LUXB_L2_PERSIST=0 disables.
+// everything else is treated as streaming when it misses.  LUXB_L2_PERSIST=0 disables.  With the cold-hub stream the
+// window covers only the hottest kColdSplitWindowMB: while that kernel runs, the persisting lines hold values it never
+// reads, and L2 is what keeps its cold segment close.
+static constexpr double kColdSplitWindowMB = 12.0;
 static int set_l2_persisting_window(luxb_graph* g, void* base, size_t bytes) {
   if (const char* env = getenv("LUXB_L2_PERSIST")) if (atoi(env) == 0) return 0;
   int max_persist = 0, max_window = 0;
@@ -906,6 +909,7 @@ static int set_l2_persisting_window(luxb_graph* g, void* base, size_t bytes) {
   LUXB_CUDA(cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, g->cfg.device));
   if (max_persist <= 0 || max_window <= 0) return 0;
   if (const char* env = getenv("LUXB_L2_WINDOW_MB")) bytes = std::min<size_t>(bytes, (size_t)(atof(env) * 1e6));  // hottest prefix only
+  else if (g->cs_on) bytes = std::min<size_t>(bytes, (size_t)(kColdSplitWindowMB * 1e6));
   size_t persist = std::min<size_t>((size_t)max_persist, bytes);
   LUXB_CUDA(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, persist));
   cudaStreamAttrValue attr{};
@@ -919,14 +923,19 @@ static int set_l2_persisting_window(luxb_graph* g, void* base, size_t bytes) {
   return 0;
 }
 
+// cold -> hub edges (PageRank, one rank) get a stream of their own when they are at least this share of the partition
+static constexpr double kColdSplitMinShare = 0.05;
+
 // Choose the hot set (largest out-degrees, at most LUXB_HOT_MB megabytes of values, default 24 MB ~ half of the H100's
 // 50 MB L2: at RMAT-27 on one H100 8 / 16 / 24 / 32 / 64 MB gave 21.4 / 15.8 / 14.2 / 16.7 / 17.3 ms per sweep) and
 // rewrite this partition's source ids as indices into the gather space Z = [hot copies in global hotness order | cold]
-// (see build.cuh).  cold = the natural-order value array, or — compact_cold, the packed exchange of PageRank on several
-// ranks — only the cold vertices that are ever gathered, in id order.
+// (see build.cuh).  cold = the natural-order value array, or — compact_cold (PageRank) — only the cold vertices that are
+// ever gathered, in id order: on several ranks the cold part of the packed exchange, on one rank a copy stored right
+// after the hot copies (Z = [hot | cold] in one buffer, refreshed with them by one gather over d_hot_order).
 static int build_hot_layout(luxb_graph* g, bool compact_cold) {
   g->hot_n = 0;
   g->packed = false;
+  g->cold_z = false;
   double hot_mb = 24.0;
   if (const char* env = getenv("LUXB_HOT_MB")) hot_mb = atof(env);
   uint64_t h_max = (uint64_t)(hot_mb * 1e6 / 4.0);
@@ -952,6 +961,20 @@ static int build_hot_layout(luxb_graph* g, bool compact_cold) {
   }
   if (above == 0 || tau > cap) return 0;
   const uint32_t H = (uint32_t)above;
+  if (compact_cold && g->P == 1) {
+    // one rank: the compact cold copy costs a refresh every iteration and pays for it in the cold-hub stream
+    // (build_panel_layout).  LUXB_CS = 0: never, 1: always, unset: when the edges out of cold vertices are at least
+    // kColdSplitMinShare of a large partition swept by the source-blocked split (the cold-hub stream needs its hubs)
+    const char* env = getenv("LUXB_CS");
+    const int cs_mode = env ? atoi(env) : -1;
+    const char* sb = getenv("LUXB_SB");
+    const char* sweep = getenv("LUXB_SWEEP");
+    const bool no_split = (sb && atoi(sb) == 0) || (sweep && !strcmp(sweep, "merge")) || g->cfg.zero_copy_edges;
+    uint64_t e_cold_src = 0;
+    for (uint32_t d = 1; d < tau; ++d) e_cold_src += (uint64_t)d * hist[d];
+    if (cs_mode == 0 || (cs_mode < 0 && (no_split || g->e_part < (1ull << 24) || (double)e_cold_src < kColdSplitMinShare * (double)g->e_part)))
+      compact_cold = false;
+  }
   uint64_t *d_keys = nullptr, *d_keys2 = nullptr;
   uint32_t *d_ids = nullptr, *d_ids2 = nullptr, *d_map = nullptr;
   unsigned int* d_cursor = nullptr;  // [0] cursor, [1 .. P] per-owner counts
@@ -988,9 +1011,9 @@ static int build_hot_layout(luxb_graph* g, bool compact_cold) {
   g->hot_off[0] = 0;
   for (int p = 0; p < g->P; ++p) g->hot_off[p + 1] = g->hot_off[p] + h_cnt[1 + p];
   LUXB_TRY(tmp.alloc(&d_map, g->nv));
-  if (compact_cold && g->P > 1) {
+  uint32_t *d_cflag = nullptr, *d_crank = nullptr;
+  if (compact_cold) {
     // cold-active vertices (0 < deg < tau), ranked in id order; owner p's share is [cold_off[p], cold_off[p+1])
-    uint32_t *d_cflag = nullptr, *d_crank = nullptr, *d_okeys = nullptr, *d_okeys2 = nullptr, *d_ranks = nullptr;
     LUXB_TRY(tmp.alloc(&d_cflag, (uint64_t)g->nv + 1));
     LUXB_TRY(tmp.alloc(&d_crank, (uint64_t)g->nv + 1));
     cold_flag_kernel<<<grid, 256, 0, g->stream>>>(g->d_deg, g->nv, tau, d_cflag);
@@ -1007,6 +1030,22 @@ static int build_hot_layout(luxb_graph* g, bool compact_cold) {
     tmp.release(d_tmp);
     g->cold_n = g->cold_off[g->P];
     gather_map_compact_kernel<<<grid, 256, 0, g->stream>>>(d_map, d_crank, g->nv, H);
+  } else {
+    gather_map_init_kernel<<<grid, 256, 0, g->stream>>>(d_map, g->nv, H);
+  }
+  if (compact_cold && g->P == 1) {
+    // d_hot_order becomes [hot order | cold-active vertices in id order]: the refresh gather fills all of Z
+    uint32_t* d_zsrc = nullptr;
+    LUXB_TRY(dmalloc(&d_zsrc, (uint64_t)H + g->cold_n + 1));
+    LUXB_CUDA(cudaMemcpyAsync(d_zsrc, g->d_hot_order, (size_t)H * 4, cudaMemcpyDeviceToDevice, g->stream));
+    pack_list_cold_kernel<<<grid, 256, 0, g->stream>>>(d_cflag, d_crank, 0, g->nv, 0, d_zsrc + H);
+    LUXB_CUDA(cudaGetLastError());
+    LUXB_CUDA(cudaStreamSynchronize(g->stream));
+    cudaFree(g->d_hot_order);
+    g->d_hot_order = d_zsrc;
+    g->cold_z = true;
+  } else if (compact_cold) {
+    uint32_t *d_okeys = nullptr, *d_okeys2 = nullptr, *d_ranks = nullptr;
     // transfer order of the hot values: grouped by owner (stable: hotness order inside a group)
     LUXB_TRY(tmp.alloc(&d_okeys, H));
     LUXB_TRY(tmp.alloc(&d_okeys2, H));
@@ -1030,8 +1069,6 @@ static int build_hot_layout(luxb_graph* g, bool compact_cold) {
     LUXB_CUDA(cudaStreamSynchronize(g->stream));
     tmp.release(d_tmp);
     g->packed = true;
-  } else {
-    gather_map_init_kernel<<<grid, 256, 0, g->stream>>>(d_map, g->nv, H);
   }
   gather_map_hot_kernel<<<grid, 256, 0, g->stream>>>(d_map, g->d_hot_order, H);
   LUXB_TRY(edge_alloc(g, &g->d_src_gather, g->e_part + 8));
@@ -1068,9 +1105,11 @@ int luxb_init(luxb_graph* g) {
       pr_init_kernel<<<grid, 256, 0, g->stream>>>(g->d_deg, g->nv, (float*)g->d_val[0]);
       LUXB_CUDA(cudaMemsetAsync(g->d_val[1], 0, (size_t)g->nv * 4, g->stream));
       if (g->hot_n) {
-        // + one whole table of slack: the panel kernel always bulk-loads full blocks (panel.cuh)
-        LUXB_TRY(dmalloc((float**)&g->d_hot, (uint64_t)g->hot_n + 65536));
-        LUXB_CUDA(cudaMemsetAsync(g->d_hot, 0, ((size_t)g->hot_n + 65536) * 4, g->stream));
+        // + the compact cold values on one rank (Z = [hot | cold]) + one whole table of slack: the panel kernel always
+        // bulk-loads full blocks (panel.cuh); only the hot prefix gets the persisting window
+        const uint64_t z_len = (uint64_t)g->hot_n + (g->cold_z ? g->cold_n : 0) + 65536;
+        LUXB_TRY(dmalloc((float**)&g->d_hot, z_len));
+        LUXB_CUDA(cudaMemsetAsync(g->d_hot, 0, z_len * 4, g->stream));
         LUXB_TRY(set_l2_persisting_window(g, g->d_hot, (size_t)g->hot_n * 4));
       }
       if (g->packed) {
@@ -1494,8 +1533,12 @@ static int build_plain_seg_layout(luxb_graph* g) {
 // from shared memory) and the main stream (everything else, gathered through L1).
 // LUXB_SB = 0 off / 1 force / unset: automatic (on when the panel would take at least a fifth of a large partition).
 // Tuning: LUXB_SB_BS (values per block), LUXB_SB_BLOCKS (max blocks), LUXB_SB_MIN_INDEG (hub threshold).
+// With the compact cold values of one rank (cold_z), the cold -> hub edges form a third stream (panel.cuh, ColdSplit):
+// LUXB_CS = 0 off / 1 force / unset: on when they are at least kColdSplitMinShare of the partition's edges;
+// LUXB_CS_SEG_MB: segment size (raised where the segments would not fit the sort key), LUXB_CS_SHAPE: its main shape.
 static int build_panel_layout(luxb_graph* g) {
   g->sb_on = false;
+  g->cs_on = false;
   const int mode = env_int("LUXB_SB", -1);
   if (mode == 0 || g->hot_n == 0 || g->e_part == 0 || g->e_part >= 0xFFFFFFFFull || g->cfg.zero_copy_edges) return 0;
   if (mode < 0 && g->e_part < (1ull << 24)) return 0;
@@ -1534,36 +1577,66 @@ static int build_panel_layout(luxb_graph* g) {
   hub_list_kernel<<<grid, 256, 0, g->stream>>>(d_flag, d_hub_idx, g->n_part, d_hub_vtx, d_hub_bits);
   LUXB_CUDA(cudaGetLastError());
 
-  // 2. edge keys: block of the source for (hot source, hub destination) edges, 255 for the rest; 3. stable sort
+  // cold segments: cold gather ids [H, H + C) cut into S segments of `seg` values, sort keys NB .. NB + S - 1 (<= 254)
+  const int cs_mode = g->cold_z ? env_int("LUXB_CS", -1) : 0;
+  ColdSplit cs{};
+  cs.hot_n = g->hot_n;
+  cs.key0 = NB;
+  uint32_t S = 0;
+  if (cs_mode != 0 && g->cold_n > 0) {
+    const char* env = getenv("LUXB_CS_SEG_MB");
+    const double seg_mb = env ? atof(env) : 24.0;
+    const uint32_t s_max = 255 - NB;
+    uint64_t seg = std::max<uint64_t>(1, (uint64_t)(seg_mb * 1e6 / 4.0));
+    seg = std::min<uint64_t>(std::max<uint64_t>(seg, (g->cold_n + s_max - 1) / s_max), g->cold_n);
+    S = (uint32_t)((g->cold_n + seg - 1) / seg);
+    if ((uint64_t)Nh * S < 0x7FFFFFF0ull) cs.seg = (uint32_t)seg;
+  }
+  uint32_t* d_cold_cnt = nullptr;
+  if (cs.seg) LUXB_TRY(tmp.alloc(&d_cold_cnt, Nh));
+
+  // 2. edge keys: block of the source for (hot source, hub destination) edges, cold segment + NB for (cold source, hub
+  // destination) edges if the cold split is on, 255 for the rest; 3. stable sort
   uint8_t *d_key = nullptr, *d_key2 = nullptr;
   uint64_t *d_pay = nullptr, *d_pay2 = nullptr;
   LUXB_TRY(tmp.alloc(&d_key, g->e_part));
   LUXB_TRY(tmp.alloc(&d_key2, g->e_part));
   LUXB_TRY(tmp.alloc(&d_pay, g->e_part));
   LUXB_TRY(tmp.alloc(&d_pay2, g->e_part));
-  edge_iota_kernel<<<grid, 256, 0, g->stream>>>(d_pay, d_key, g->e_part);
-  hub_key_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, g->d_src_gather, d_hub_vtx, Nh, n_src, bs, d_key, d_pay, d_cov);
-  LUXB_CUDA(cudaGetLastError());
+  unsigned long long* d_hist = nullptr;
+  LUXB_TRY(tmp.alloc(&d_hist, 256));
+  unsigned long long hist[256];
+  for (;;) {
+    edge_iota_kernel<<<grid, 256, 0, g->stream>>>(d_pay, d_key, g->e_part);
+    hub_key_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, g->d_src_gather, d_hub_vtx, Nh, n_src, bs, d_key, d_pay, d_cov, cs, d_cold_cnt);
+    LUXB_CUDA(cudaMemsetAsync(d_hist, 0, 256 * 8, g->stream));
+    key_hist_kernel<<<grid, 256, 0, g->stream>>>(d_key, g->e_part, d_hist);
+    LUXB_CUDA(cudaGetLastError());
+    LUXB_CUDA(cudaMemcpyAsync(hist, d_hist, sizeof(hist), cudaMemcpyDeviceToHost, g->stream));
+    LUXB_CUDA(cudaStreamSynchronize(g->stream));
+    uint64_t e_cs = 0;
+    for (uint32_t s = 0; s < S; ++s) e_cs += hist[NB + s];
+    if (cs.seg == 0 || cs_mode > 0 || (e_cs > 0 && (double)e_cs >= kColdSplitMinShare * (double)g->e_part)) break;
+    cs.seg = 0;  // automatic and too few cold -> hub edges: key again without the cold split
+  }
+  if (cs.seg == 0) S = 0;
   tb = 0;
   LUXB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_key, d_key2, d_pay, d_pay2, (long long)g->e_part, 0, 8, g->stream));
   LUXB_TRY(tmp.alloc((char**)&d_scan_tmp, tb + 256));
   LUXB_CUDA(cub::DeviceRadixSort::SortPairs(d_scan_tmp, tb, d_key, d_key2, d_pay, d_pay2, (long long)g->e_part, 0, 8, g->stream));
-  unsigned long long* d_hist = nullptr;
-  LUXB_TRY(tmp.alloc(&d_hist, 256));
-  LUXB_CUDA(cudaMemsetAsync(d_hist, 0, 256 * 8, g->stream));
-  key_hist_kernel<<<grid, 256, 0, g->stream>>>(d_key2, g->e_part, d_hist);
-  LUXB_CUDA(cudaGetLastError());
-  unsigned long long hist[256];
-  LUXB_CUDA(cudaMemcpyAsync(hist, d_hist, sizeof(hist), cudaMemcpyDeviceToHost, g->stream));
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
   tmp.release(d_scan_tmp);
   tmp.release(d_key);
   tmp.release(d_pay);
-  uint64_t e_cov = 0;
+  uint64_t e_cov = 0, e_cold = 0;
   for (uint32_t b = 0; b < NB; ++b) e_cov += hist[b];
+  for (uint32_t s = 0; s < S; ++s) e_cold += hist[NB + s];
   const uint64_t e_main = hist[255];
-  if (e_cov + e_main != g->e_part) { set_error("panel split lost edges (%llu + %llu != %llu)", (unsigned long long)e_cov,
-                                               (unsigned long long)e_main, (unsigned long long)g->e_part); return LUXB_ERR_STATE; }
+  if (e_cov + e_cold + e_main != g->e_part) {
+    set_error("panel split lost edges (%llu + %llu + %llu != %llu)", (unsigned long long)e_cov, (unsigned long long)e_cold,
+              (unsigned long long)e_main, (unsigned long long)g->e_part);
+    return LUXB_ERR_STATE;
+  }
   if (e_cov == 0 || (mode < 0 && e_cov < g->e_part / 5)) return 0;
 
   // 4. panel CSC over virtual vertices (block b, hub h) -> index b * Nh + h: offsets + per-vertex in-degree
@@ -1598,13 +1671,49 @@ static int build_panel_layout(luxb_graph* g) {
   tmp.release(d_vrow);
   tmp.release(d_src16);
 
+  // 4b. cold-hub CSC over virtual vertices (segment s, hub h) -> index s * Nh + h, gather ids unchanged: one block,
+  // no padding between segments (its kernel claims stages in order, so the SMs move through the segments together)
+  if (S) {
+    const uint32_t NVc = Nh * S;
+    uint32_t *d_cids = nullptr, *d_ccount = nullptr;
+    uint64_t* d_crow = nullptr;
+    LUXB_TRY(tmp.alloc(&d_cids, e_cold + 8));
+    LUXB_TRY(tmp.alloc(&d_ccount, (uint64_t)NVc + 1));
+    LUXB_CUDA(cudaMemsetAsync(d_ccount, 0, ((size_t)NVc + 1) * 4, g->stream));
+    cold_fill_kernel<<<grid, 256, 0, g->stream>>>(d_key2 + e_cov, d_pay2 + e_cov, e_cold, g->d_src_gather, NB, Nh, d_cids, d_ccount);
+    LUXB_CUDA(cudaGetLastError());
+    LUXB_TRY(tmp.alloc(&d_crow, (uint64_t)NVc + 4));
+    widen_u32_to_u64_kernel<<<grid, 256, 0, g->stream>>>(d_ccount, d_crow, NVc);
+    tb = 0;
+    LUXB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb, d_crow, d_crow, (int)NVc, g->stream));
+    LUXB_TRY(tmp.alloc((char**)&d_scan_tmp, tb + 256));
+    LUXB_CUDA(cub::DeviceScan::InclusiveSum(d_scan_tmp, tb, d_crow, d_crow, (int)NVc, g->stream));
+    LUXB_CUDA(cudaStreamSynchronize(g->stream));
+    tmp.release(d_scan_tmp);
+    tmp.release(d_ccount);
+    g->cs_shape = env_int("LUXB_CS_SHAPE", g->seg_main_shape);
+    if (g->cs_shape < 0 || g->cs_shape >= kNumSegMain) g->cs_shape = 0;
+    const SegShapeInfo cshp = kSegMainInfo[g->cs_shape];
+    StreamBlocks cblk{};
+    cblk.n_blocks = 1;
+    cblk.vfirst[0] = 0; cblk.vfirst[1] = NVc;
+    cblk.ebase[0] = 0; cblk.ebase[1] = e_cold;
+    LUXB_TRY((build_seg_stream<uint32_t, uint32_t>(g, g->sb_cold, d_crow, NVc, d_cids, e_cold, cblk, (uint32_t)cshp.stage_edges,
+                                                   (uint32_t)cshp.piece, 0, false, nullptr, nullptr)));
+    tmp.release(d_crow);
+    tmp.release(d_cids);
+    // raw cold-hub sums: (segment, hub) pairs without edges keep the identity (0: PageRank only)
+    LUXB_TRY(dmalloc(&g->d_cs_partial, (uint64_t)NVc + 1));
+    LUXB_CUDA(cudaMemsetAsync(g->d_cs_partial, 0, ((size_t)NVc + 1) * 4, g->stream));
+  }
+
   // 5. main stream: what is left, in the original (dst, src) order
   uint32_t* d_main_src = nullptr;
   uint64_t* d_main_row = nullptr;
   LUXB_TRY(tmp.alloc(&d_main_src, e_main + 8));
-  main_fill_kernel<<<grid, 256, 0, g->stream>>>(d_pay2 + e_cov, e_main, g->d_src_gather, d_main_src);
+  main_fill_kernel<<<grid, 256, 0, g->stream>>>(d_pay2 + e_cov + e_cold, e_main, g->d_src_gather, d_main_src);
   LUXB_TRY(tmp.alloc(&d_main_row, (uint64_t)g->n_part + 4));
-  main_indeg_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, g->n_part, d_flag, d_hub_idx, d_cov, d_main_row);
+  main_indeg_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, g->n_part, d_flag, d_hub_idx, d_cov, S ? d_cold_cnt : nullptr, d_main_row);
   LUXB_CUDA(cudaGetLastError());
   tb = 0;
   LUXB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb, d_main_row, d_main_row, (int)g->n_part, g->stream));
@@ -1639,13 +1748,18 @@ static int build_panel_layout(luxb_graph* g) {
   g->sb_bs = bs;
   g->sb_n_src = n_src;
   g->sb_on = true;
+  g->cs_on = S > 0;
+  g->cs_n_seg = S;
+  g->cs_seg = cs.seg;
   g->stats.panel_edges = e_cov;
   g->stats.panel_hubs = Nh;
   g->stats.panel_blocks = NB;
+  g->stats.cold_hub_edges = e_cold;
+  g->stats.cold_hub_segments = S;
   if (g->cfg.verbose)
     printf("[luxb rank %d] source-blocked sweep: %u hub destinations (in-degree >= %u) x %u blocks of %u hot sources; panel %llu edges "
-           "(%.1f %%), main %llu edges\n", g->cfg.rank, Nh, min_indeg, NB, bs, (unsigned long long)e_cov, 100.0 * e_cov / g->e_part,
-           (unsigned long long)e_main);
+           "(%.1f %%), cold-hub %llu edges (%u segments of %u values), main %llu edges\n", g->cfg.rank, Nh, min_indeg, NB, bs,
+           (unsigned long long)e_cov, 100.0 * e_cov / g->e_part, (unsigned long long)e_cold, S, cs.seg, (unsigned long long)e_main);
   return 0;
 }
 
@@ -1661,6 +1775,7 @@ static int build_seg_sweep(luxb_graph* g) {
   g->seg_panel_shape = env_int("LUXB_SEG_PANEL_SHAPE", 1);
   if (g->seg_panel_shape < 0 || g->seg_panel_shape >= kNumSegPanel) g->seg_panel_shape = 0;
   LUXB_TRY(build_panel_layout(g));
+  if (!g->cs_on) free_layout(g->sb_cold);
   if (!g->sb_on) {
     free_layout(g->sb_panel);
     LUXB_TRY(build_plain_seg_layout(g));
@@ -1772,6 +1887,32 @@ static int sweep_seg(luxb_graph* g, const typename Prog::Vertex* x_nat, const ty
     LUXB_TRY(launch_fixup(g, pa.p, PL));
     pt_mark(g, 1);
   }
+  if (g->cs_on) {
+    // cold-hub stream: raw partial per (cold segment, hub); its gathers all index the compact cold values, which it
+    // loads with evict_normal (l2_hints = 0): the current segment is meant to stay in L2 while the SMs sweep it
+    PullLayout& CL = g->sb_cold;
+    SegArgs<Prog> ca{};
+    fill_seg_args(ca, CL);
+    ca.p.x_old = x_cold;
+    ca.p.x_hot = reinterpret_cast<const typename Prog::Vertex*>(g->d_hot);
+    ca.p.hot_n = g->hot_n;
+    ca.p.out = reinterpret_cast<typename Prog::Vertex*>(g->d_cs_partial);
+    ca.p.raw_out = 1;
+    ca.p.l2_hints = 0;
+    ca.p.prm = prm;
+    ca.tile_counter = reinterpret_cast<uint32_t*>(g->d_counters + 4);
+    LUXB_CUDA(cudaMemsetAsync(ca.tile_counter, 0, 4, g->stream));
+    switch (g->cs_shape) {
+#define LUXB_CASE_CSHAPE(id, warps, stages, rounds) \
+      case id: LUXB_TRY((launch_seg_shape<Prog, SegMain##id>(g, ca, g->pull_ctas))); break;
+      LUXB_SEG_MAIN_SHAPES(LUXB_CASE_CSHAPE)
+      default: set_error("bad cold-hub shape"); return LUXB_ERR_STATE;
+    }
+    g->stats.kernel_launches++;
+    pt_mark(g, 9);
+    LUXB_TRY(launch_fixup(g, ca.p, CL));
+    pt_mark(g, 1);
+  }
   LUXB_TRY((launch_seg_main<Prog>(g, g->sb_main, x_nat, x_cold, out_local, out_buffer, prm, g->sb_on ? g->d_hub_bits : nullptr)));
   LUXB_TRY(kt_end(g));
   if (g->sb_on) {
@@ -1782,6 +1923,8 @@ static int sweep_seg(luxb_graph* g, const typename Prog::Vertex* x_nat, const ty
     ca.row_left = g->row_left;
     ca.pb = g->sb_pb;
     ca.partial = reinterpret_cast<const Acc*>(g->d_sb_partial);
+    ca.cold_partial = reinterpret_cast<const Acc*>(g->d_cs_partial);
+    ca.n_cold_seg = g->cs_on ? g->cs_n_seg : 0;
     ca.x_nat = x_nat;
     ca.out = out_local;
     ca.prm = prm;
@@ -1807,7 +1950,8 @@ static int pagerank_publish(luxb_graph* g, float* x_new) {
   if (g->P == 1 || !g->packed) {
     if (g->P > 1) { LUXB_TRY(allgather_slices(g, x_new, 4)); pt_mark(g, 3); }  // graphs without a hot set (tiny): plain all-gather
     if (g->hot_n) {
-      hot_refresh_kernel<float><<<grid_for(g->hot_n, 256, grid), 256, 0, g->stream>>>((float*)g->d_hot, x_new, g->d_hot_order, 0, g->hot_n);
+      const uint32_t z_n = g->hot_n + (g->cold_z ? g->cold_n : 0);
+      hot_refresh_kernel<float><<<grid_for(z_n, 256, grid), 256, 0, g->stream>>>((float*)g->d_hot, x_new, g->d_hot_order, 0, z_n);
       LUXB_CUDA(cudaGetLastError());
       g->stats.kernel_launches++;
       pt_mark(g, 2);
@@ -1920,7 +2064,7 @@ static int pagerank_iteration(luxb_graph* g) {
   prm.deg = g->d_deg;
   float* x_old = (float*)g->d_val[g->cur];
   float* x_new = (float*)g->d_val[1 - g->cur];
-  const float* x_cold = g->packed ? g->d_xt[g->cur_xt] + g->xt_hot_chunk * g->P : x_old;
+  const float* x_cold = g->packed ? g->d_xt[g->cur_xt] + g->xt_hot_chunk * g->P : g->cold_z ? (const float*)g->d_hot + g->hot_n : x_old;
   if (g->seg_on) {
     LUXB_TRY((sweep_seg<PageRankProgram>(g, x_old, x_cold, x_new + g->row_left, 1 - g->cur, prm)));
   } else {
@@ -2425,7 +2569,7 @@ int luxb_debug_gather_ms(luxb_graph* g, int packed, float* ms_out) {
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
   const bool use_hot = packed && g->hot_n;
   const uint32_t* idx = use_hot ? g->d_src_gather : g->d_src;
-  const float* nat = (const float*)g->d_val[g->cur];
+  const float* nat = use_hot && g->cold_z ? (const float*)g->d_hot + g->hot_n : (const float*)g->d_val[g->cur];
   const uint32_t hn = use_hot ? g->hot_n : 0;
   float best = 1e30f;
   for (int r = 0; r < 4; ++r) {
@@ -2494,6 +2638,8 @@ void luxb_close(luxb_graph* g) {
   }
   free_layout(g->sb_main);
   free_layout(g->sb_panel);
+  free_layout(g->sb_cold);
+  if (g->d_cs_partial) cudaFree(g->d_cs_partial);
   if (g->base_view.d_chain) cudaFree(g->base_view.d_chain);
   if (g->d_hub_vtx) cudaFree(g->d_hub_vtx);
   if (g->d_hub_bits) cudaFree(g->d_hub_bits);

@@ -56,27 +56,51 @@ __global__ void edge_iota_kernel(uint64_t* __restrict__ payload, uint8_t* __rest
   }
 }
 
-// one warp per hub vertex: edges whose (hot-packed) source id lies below n_src get key = block, payload = (h, e)
+// Cold-hub split (PageRank on one rank, where the cold values are compacted right after the hot copies): edges from a
+// COLD source (gather id >= H) into a hub move into a third flagged stream, ordered by cold source segment of `seg`
+// values: virtual vertex s * Nh + h.  Its kernel claims stages in order, so at any time all SMs gather from about one
+// segment, which stays in L2 beside the persisting hot copies, instead of from the whole cold array at random.  Only
+// hub destinations are split this way: their partials cost Nh * S slots, where splitting every destination would cost
+// n_part * S.
+struct ColdSplit {
+  uint32_t hot_n;    // first cold gather id (H)
+  uint32_t seg;      // cold values per segment; 0 = no cold-hub split
+  uint32_t key0;     // sort key of segment 0 (= number of panel blocks)
+};
+
+// one warp per hub vertex: edges whose (hot-packed) source id lies below n_src get key = block, payload = (h, e);
+// with the cold split on, edges whose source is cold get key = cs.key0 + segment
 __global__ void hub_key_kernel(const uint64_t* __restrict__ row_end_rel, const uint32_t* __restrict__ src_gather,
                                const uint32_t* __restrict__ hub_vtx, uint32_t n_hub, uint32_t n_src, uint32_t bs,
-                               uint8_t* __restrict__ key, uint64_t* __restrict__ payload, uint32_t* __restrict__ cov_count) {
+                               uint8_t* __restrict__ key, uint64_t* __restrict__ payload, uint32_t* __restrict__ cov_count,
+                               const ColdSplit cs, uint32_t* __restrict__ cold_count) {
   const unsigned lane = threadIdx.x & 31;
   const uint64_t warps_total = ((uint64_t)gridDim.x * blockDim.x) >> 5;
   for (uint64_t h = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; h < n_hub; h += warps_total) {
     const uint32_t v = hub_vtx[h];
     const uint64_t b = v == 0 ? 0 : row_end_rel[v - 1], e = row_end_rel[v];
-    uint32_t cnt = 0;
+    uint32_t cnt = 0, ccnt = 0;
     for (uint64_t k = b + lane; k < e; k += 32) {
       const uint32_t id = src_gather[k];
       if (id < n_src) {
         key[k] = (uint8_t)(id / bs);
         payload[k] = (h << 32) | k;
         ++cnt;
+      } else if (cs.seg != 0 && id >= cs.hot_n) {
+        key[k] = (uint8_t)(cs.key0 + (id - cs.hot_n) / cs.seg);
+        payload[k] = (h << 32) | k;
+        ++ccnt;
       }
     }
 #pragma unroll
-    for (int off = 16; off; off >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, off);
-    if (lane == 0) cov_count[h] = cnt;
+    for (int off = 16; off; off >>= 1) {
+      cnt += __shfl_xor_sync(0xffffffffu, cnt, off);
+      ccnt += __shfl_xor_sync(0xffffffffu, ccnt, off);
+    }
+    if (lane == 0) {
+      cov_count[h] = cnt;
+      if (cs.seg != 0) cold_count[h] = ccnt;
+    }
   }
 }
 
@@ -109,30 +133,45 @@ __global__ void panel_fill_kernel(const uint8_t* __restrict__ key_sorted, const 
   }
 }
 
+// sorted (by segment, stable) cold-hub edges -> their gather ids unchanged + per-virtual-vertex (s * Nh + h) in-degree
+__global__ void cold_fill_kernel(const uint8_t* __restrict__ key_sorted, const uint64_t* __restrict__ payload_sorted, uint64_t e_cold,
+                                 const uint32_t* __restrict__ src_gather, uint32_t key0, uint32_t n_hub, uint32_t* __restrict__ ids,
+                                 uint32_t* __restrict__ vcount) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < e_cold; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t p = payload_sorted[i];
+    const uint32_t e = (uint32_t)p, h = (uint32_t)(p >> 32);
+    ids[i] = src_gather[e];
+    atomicAdd(vcount + (uint64_t)(key_sorted[i] - key0) * n_hub + h, 1u);
+  }
+}
+
 __global__ void main_fill_kernel(const uint64_t* __restrict__ payload_sorted, uint64_t e_main, const uint32_t* __restrict__ src_gather,
                                  uint32_t* __restrict__ main_src) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < e_main; i += (uint64_t)gridDim.x * blockDim.x)
     main_src[i] = src_gather[(uint32_t)payload_sorted[i]];
 }
 
-// in-degree of every local vertex inside the MAIN CSC = its in-degree minus the edges that moved to the panel
+// in-degree of every local vertex inside the MAIN CSC = its in-degree minus the edges that moved to the panel and (if
+// cold_count is given) to the cold-hub stream
 __global__ void main_indeg_kernel(const uint64_t* __restrict__ row_end_rel, uint32_t n_part, const uint32_t* __restrict__ flag,
                                   const uint32_t* __restrict__ hub_idx, const uint32_t* __restrict__ cov_count,
-                                  uint64_t* __restrict__ out) {
+                                  const uint32_t* __restrict__ cold_count, uint64_t* __restrict__ out) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_part; i += (uint64_t)gridDim.x * blockDim.x) {
     uint64_t d = row_end_rel[i] - (i == 0 ? 0 : row_end_rel[i - 1]);
-    if (flag[i]) d -= cov_count[hub_idx[i]];
+    if (flag[i]) d -= cov_count[hub_idx[i]] + (cold_count ? cold_count[hub_idx[i]] : 0u);
     out[i] = d;
   }
 }
 
-// ---- per-iteration: hubs = main raw sum + panel partials, fp64, fixed order; then update() -------------------------
+// ---- per-iteration: hubs = main raw sum + panel partials + cold-segment partials, fp64, fixed order; then update() ---
 template <class Prog>
 struct CombineArgs {
   const uint32_t* hub_vtx;   // [n_hub] local vertex ids
   uint32_t n_hub, n_blocks, row_left;
   PanelBases pb;
   const typename Prog::Acc* partial;  // [NV] raw panel reductions
+  const typename Prog::Acc* cold_partial;  // [n_cold_seg * n_hub] raw cold-hub reductions, slot s * n_hub + h
+  uint32_t n_cold_seg;
   const typename Prog::Vertex* x_nat; // natural-order values of the previous iteration (update()'s old value)
   typename Prog::Vertex* out;  // [n_part] local; holds the main kernel's RAW sum for hub vertices on entry
   typename Prog::Params prm;
@@ -146,6 +185,7 @@ __global__ void combine_hub_kernel(const __grid_constant__ CombineArgs<Prog> a) 
     memcpy(&raw0, &a.out[v], sizeof(raw0));  // the main sweep left its RAW reduction in the value slot
     typename Prog::Wide t = Prog::widen(raw0);
     for (uint32_t b = 0; b < a.n_blocks; ++b) t = Prog::wcombine(t, Prog::widen(a.partial[a.pb.vbase[b] + h]));
+    for (uint32_t s = 0; s < a.n_cold_seg; ++s) t = Prog::wcombine(t, Prog::widen(a.cold_partial[(uint64_t)s * a.n_hub + h]));
     const typename Prog::Vertex oldv = Prog::kNeedsOld ? a.x_nat[a.row_left + v] : typename Prog::Vertex();
     const typename Prog::Vertex nv_ = Prog::update(a.row_left + v, Prog::narrow(t), oldv, a.prm);
     a.out[v] = nv_;

@@ -99,7 +99,7 @@ struct luxb_graph {
   uint32_t hot_n = 0;
   void* d_hot = nullptr;             // [hot_n] hot copies (single buffer: refreshed in place after every iteration)
   uint32_t hot_off[LUXB_MAX_PARTS + 1]{};  // hot slots owned by partition p: [hot_off[p], hot_off[p+1])
-  uint32_t* d_hot_order = nullptr;   // [hot_n] vertex id held by each hot slot (descending out-degree)
+  uint32_t* d_hot_order = nullptr;   // [hot_n (+ cold_n if cold_z)] vertex id held by each hot slot (descending out-degree)
   uint32_t* d_src_gather = nullptr;  // [e_part + 8] source ids rewritten as indices into Z
   // packed exchange (PageRank, nranks > 1): transfer arrays XT[2] = [hot by owner (hot_n) | cold-active by id (cold_n)]
   bool packed = false;
@@ -170,6 +170,14 @@ struct luxb_graph {
   uint32_t* d_sb_partial = nullptr;  // [NV] raw panel reductions (4-byte Acc of the app's program)
   luxb::PanelBases sb_pb{};
   uint32_t sb_super_end[luxb::kPanelMaxBlocks]{};
+  // cold-hub stream (PageRank, one rank): cold source segment x hub destination, gathered through L1 from an L2-sized
+  // segment of the compact cold values (panel.cuh, ColdSplit)
+  bool cold_z = false;             // one rank: d_hot = Z = [hot copies | cold-active values in id order], d_hot_order covers both
+  bool cs_on = false;
+  int cs_shape = 0;                // main shape of the cold-hub stream's kernel (LUXB_CS_SHAPE)
+  PullLayout sb_cold;
+  uint32_t cs_n_seg = 0, cs_seg = 0;
+  uint32_t* d_cs_partial = nullptr;  // [cs_n_seg * sb_n_hub] raw cold-hub reductions
 
   // launch configuration resolved once at open time (no getenv / function-static state on the hot path)
   int pull_ctas = 3;
