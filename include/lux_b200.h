@@ -48,8 +48,23 @@ typedef enum {
   LUXB_PAGERANK = 0, /* pagerank/   — pull model, f32 vertex value (rank / out-degree) */
   LUXB_CC = 1,       /* components/ — push/pull hybrid, u32 label, max */
   LUXB_SSSP = 2,     /* sssp/       — push/pull hybrid, u32 hop distance, min(+1), INF = nv */
-  LUXB_COLFILTER = 3 /* col_filter/ — pull model, float[20] vertex value */
+  LUXB_COLFILTER = 3, /* col_filter/ — pull model, float[20] vertex value */
+  LUXB_SSSP_WEIGHTED = 4 /* weighted SSSP (no reference counterpart) — push/pull hybrid, u32 distance, INF = LUXB_DIST_INF */
 } luxb_app;
+
+/* Weighted SSSP (LUXB_SSSP_WEIGHTED):
+ *  - weights are the CSC's i32 per-edge weights, in CSC edge order; they must be >= 0 (zero is allowed): a negative
+ *    weight fails the open with LUXB_ERR_ARG.  The graph must carry weights (csc->weight, or the .lux i32 trailer);
+ *    luxb_open_rmat generates them (see there), luxb_open_bipartite uses its ratings 1..5;
+ *  - distances are u32; INF = LUXB_DIST_INF (not nv: real distances can exceed nv).  D[start] = 0, every other INF;
+ *  - relaxation cand = sat_add(D[u], w) = min(D[u] + w, INF), computed without wrap-around: INF + w = INF, and a
+ *    distance that would reach 2^32 - 1 reads as unreachable;
+ *  - otherwise SSSP's structure: Jacobi iterations, pull when the global active count > nv/16 (the merge-path sweep),
+ *    push otherwise, the same frontier representation rules, halt on zero active.  Labels after every iteration do not
+ *    depend on the direction taken, so labels, per-iteration active counts and pull flags are deterministic;
+ *  - luxb_check counts the in-edges with D[u] != INF && D[v] > sat_add(D[u], w).
+ * LUXB_SSSP keeps its hop-count semantics even when the CSC passed to it carries weights. */
+#define LUXB_DIST_INF 0xFFFFFFFFu
 
 typedef enum {
   LUXB_EXCHANGE_NCCL = 0, /* library collectives only: PageRank packs its share and broadcasts the two ranges of every
@@ -72,7 +87,7 @@ typedef struct {
   luxb_eid ne;
   const luxb_eid* row_end;
   const luxb_vid* src;
-  const int32_t* weight; /* NULL unless app == LUXB_COLFILTER */
+  const int32_t* weight; /* needed by LUXB_COLFILTER and LUXB_SSSP_WEIGHTED; ignored by the other apps */
 } luxb_csc;
 
 typedef struct {
@@ -103,7 +118,10 @@ int luxb_open_csc(const luxb_csc* csc, const luxb_config* cfg, luxb_graph** out)
 int luxb_open_file(const char* lux_path, const luxb_config* cfg, luxb_graph** out);
 /* Synthetic inputs generated ON THE DEVICE (no reference counterpart; SURVEY §8d): deterministic counter-based
  * RMAT (a,b,c,d = .57,.19,.19,.05), endpoints >= nv rejected, canonical (dst,src)-sorted CSC.  Bit-identical to
- * oracle lo_gen_rmat_csc.  Every rank generates the edge stream and keeps only its own partition. */
+ * oracle lo_gen_rmat_csc.  Every rank generates the edge stream and keeps only its own partition.
+ * app == LUXB_SSSP_WEIGHTED: every edge also gets a directed weight in [1, 255] that depends only on (seed, src, dst):
+ *   w = 1 + (splitmix64(splitmix64(seed ^ 0x9E3779B97F4A7C15) ^ (dst << 32 | src)) >> 32) % 255
+ * (bit-identical to the weighted-SSSP test oracle, tests/weighted_oracle.c wo_rmat_weight). */
 int luxb_open_rmat(int scale, luxb_vid nv, luxb_eid ne, uint64_t seed, const luxb_config* cfg, luxb_graph** out);
 /* NetFlix-like bipartite ratings graph, every rating stored in both directions (ne = 2*ratings), int weights 1..5. */
 int luxb_open_bipartite(luxb_vid users, luxb_vid items, luxb_eid ratings, uint64_t seed, const luxb_config* cfg,
@@ -174,7 +192,8 @@ int luxb_set_values(luxb_graph* g, const void* host_in, size_t bytes);
 int luxb_set_local_values(luxb_graph* g, const void* host_in, size_t bytes);
 int luxb_get_local_values(luxb_graph* g, void* host_out, size_t bytes);
 /* CheckTask / check_kernel invariants (components_gpu.cu:768-837, sssp_gpu.cu:773-843): number of violating
- * edges over this rank's partition; PageRank / col_filter have no check in the reference -> LUXB_ERR_ARG. */
+ * edges over this rank's partition; PageRank / col_filter have no check in the reference -> LUXB_ERR_ARG.
+ * LUXB_SSSP_WEIGHTED: in-edges with D[u] != LUXB_DIST_INF && D[v] > sat_add(D[u], w). */
 int luxb_check(luxb_graph* g, uint64_t* mistakes_out);
 
 typedef struct {

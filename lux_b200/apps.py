@@ -2,11 +2,11 @@
 
 pagerank   : pagerank/pagerank.cc:105-118     (-ni fixed iterations)
 components : components/components.cc:108-135 (run until no partition reports an active vertex)
-sssp       : sssp/sssp.cc                     (same loop, -start)
+sssp       : sssp/sssp.cc                     (same loop, -start; with weights: weighted SSSP, ours)
 colfilter  : col_filter/colfilter.cc:71-81    (-ni fixed iterations)
 Single-rank convenience wrappers; multi-GPU callers drive LuxGraph directly (see bench.py).
 """
-from .binding import LuxGraph, APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER
+from .binding import LuxGraph, APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED
 
 
 def pagerank(row_end, src, num_iter=10, device=0):
@@ -27,8 +27,11 @@ def components(row_end, src, device=0, check=False):
         return out
 
 
-def sssp(row_end, src, start=0, device=0, check=False):
-    with LuxGraph.from_csc(row_end, src, app=APP_SSSP, start=start, device=device) as g:
+def sssp(row_end, src, start=0, device=0, check=False, weight=None):
+    """Hop counts (INF = nv), or with `weight` (i32 per edge, CSC order, >= 0) weighted shortest-path distances
+    (INF = DIST_INF = 2^32 - 1, sums saturate at INF)."""
+    app = APP_SSSP if weight is None else APP_SSSP_WEIGHTED
+    with LuxGraph.from_csc(row_end, src, weight, app=app, start=start, device=device) as g:
         g.init()
         iters = g.run_to_convergence()
         out = dict(labels=g.values(), iters=iters, trace=g.trace())

@@ -6,7 +6,8 @@ import numpy as np
 
 from . import build as _build
 
-APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER = 0, 1, 2, 3
+APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED = 0, 1, 2, 3, 4
+DIST_INF = 0xFFFFFFFF  # APP_SSSP_WEIGHTED: distance of an unreachable vertex (LUXB_DIST_INF)
 EXCHANGE_NCCL, EXCHANGE_P2P, EXCHANGE_P2P_FUSED = 0, 1, 2
 DENSE_BITMAP, SPARSE_QUEUE = 0x1234567, 0x7654321
 CF_K = 20
@@ -117,7 +118,8 @@ def convert_edgelist(edge_list_path, lux_path, nv, ne):
          "luxb_convert_edgelist")
 
 
-_VDTYPE = {APP_PAGERANK: np.float32, APP_CC: np.uint32, APP_SSSP: np.uint32, APP_COLFILTER: np.float32}
+_VDTYPE = {APP_PAGERANK: np.float32, APP_CC: np.uint32, APP_SSSP: np.uint32, APP_COLFILTER: np.float32,
+           APP_SSSP_WEIGHTED: np.uint32}
 
 
 class LuxGraph:
@@ -167,12 +169,13 @@ class LuxGraph:
         return cls(h, app, rank, nranks)
 
     @classmethod
-    def from_bipartite(cls, users, items, ratings, seed, rank=0, nranks=1, device=0, exchange=EXCHANGE_NCCL, balanced=False):
-        cfg = cls._cfg(APP_COLFILTER, rank, nranks, device, 0, exchange, False, False, balanced)
+    def from_bipartite(cls, users, items, ratings, seed, rank=0, nranks=1, device=0, exchange=EXCHANGE_NCCL, balanced=False,
+                       app=APP_COLFILTER, start=0):
+        cfg = cls._cfg(app, rank, nranks, device, start, exchange, False, False, balanced)
         h = C.c_void_p()
         _chk(load_library().luxb_open_bipartite(C.c_uint32(users), C.c_uint32(items), C.c_uint64(ratings),
                                                 C.c_uint64(seed), C.byref(cfg), C.byref(h)), "luxb_open_bipartite")
-        return cls(h, APP_COLFILTER, rank, nranks)
+        return cls(h, app, rank, nranks)
 
     # ---- partition table ----------------------------------------------------------------------------------
     def bounds(self):

@@ -184,11 +184,16 @@ static bool use_balanced_split(const luxb_config* cfg) {
 
 static int check_config(const luxb_config* cfg) {
   LUXB_ARG(cfg != nullptr, "config is NULL");
-  LUXB_ARG(cfg->app >= LUXB_PAGERANK && cfg->app <= LUXB_COLFILTER, "unknown app %d", (int)cfg->app);
+  LUXB_ARG(cfg->app >= LUXB_PAGERANK && cfg->app <= LUXB_SSSP_WEIGHTED, "unknown app %d", (int)cfg->app);
   LUXB_ARG(cfg->nranks >= 1 && cfg->nranks <= LUXB_MAX_PARTS, "nranks %d out of range [1,%d]", cfg->nranks, LUXB_MAX_PARTS);
   LUXB_ARG(cfg->rank >= 0 && cfg->rank < cfg->nranks, "rank %d out of range", cfg->rank);
   return 0;
 }
+
+// the push/pull hybrid apps: u32 labels in one replica (d_val[0]), frontier engine, luxb_check
+static bool is_label_app(luxb_app app) { return app == LUXB_CC || app == LUXB_SSSP || app == LUXB_SSSP_WEIGHTED; }
+// apps that read the CSC's edge weights
+static bool uses_weights(luxb_app app) { return app == LUXB_COLFILTER || app == LUXB_SSSP_WEIGHTED; }
 
 static int graph_begin(const luxb_config* cfg, luxb_graph** out) {
   LUXB_TRY(check_config(cfg));
@@ -312,8 +317,16 @@ static int upload_slice(luxb_graph* g, const uint64_t* row_end_slice_abs, const 
   unsigned long long bad = 0;
   LUXB_CUDA(cudaMemcpyAsync(&bad, d_bad, 8, cudaMemcpyDeviceToHost, g->stream));
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  unsigned long long neg = 0;
+  if (g->cfg.app == LUXB_SSSP_WEIGHTED && g->e_part) {  // shortest paths need w >= 0 (checked the same way, on the device)
+    LUXB_CUDA(cudaMemsetAsync(d_bad, 0, 8, g->stream));
+    negative_weight_kernel<<<g->num_sms * 8, 256, 0, g->stream>>>(g->d_weight, g->e_part, d_bad);
+    LUXB_CUDA(cudaMemcpyAsync(&neg, d_bad, 8, cudaMemcpyDeviceToHost, g->stream));
+    LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  }
   LUXB_CUDA(cudaFree(d_tmp));
   LUXB_ARG(bad == 0, "%llu source ids of this rank's slice are >= nv (%u)", bad, g->nv);
+  LUXB_ARG(neg == 0, "%llu edge weights of this rank's slice are negative (weighted SSSP needs w >= 0)", neg);
   return finish_layout(g);
 }
 
@@ -339,13 +352,14 @@ int luxb_open_csc(const luxb_csc* csc, const luxb_config* cfg, luxb_graph** out)
   LUXB_ARG(csc && csc->row_end && (csc->src || csc->ne == 0), "csc arrays are NULL");
   LUXB_TRY(check_config(cfg));
   LUXB_ARG(cfg->app != LUXB_COLFILTER || csc->weight, "col_filter needs edge weights (EDGE_WEIGHT, col_filter/app.h:22)");
+  LUXB_ARG(cfg->app != LUXB_SSSP_WEIGHTED || csc->weight || csc->ne == 0, "weighted SSSP needs edge weights");
   LUXB_TRY(validate_row_end(csc->nv, csc->ne, csc->row_end));
   luxb_graph* g = nullptr;
   int rc = graph_begin(cfg, &g);
   if (rc) { if (g) luxb_close(g); return rc; }
   g->nv = csc->nv;
   g->ne = csc->ne;
-  g->weighted = cfg->app == LUXB_COLFILTER;
+  g->weighted = uses_weights(cfg->app);
   g->parts_found = host_partition(g->nv, g->ne, csc->row_end, g->P, g->ref_rl, g->ref_np, g->ref_cl);
   if (use_balanced_split(cfg)) host_balanced_partition(g->nv, g->ne, csc->row_end, g->P, g->rl, g->np, g->cl);
   else for (int p = 0; p < g->P; ++p) { g->rl[p] = g->ref_rl[p]; g->np[p] = g->ref_np[p]; g->cl[p] = g->ref_cl[p]; }
@@ -378,7 +392,7 @@ int luxb_open_file(const char* path, const luxb_config* cfg, luxb_graph** out) {
   if (rc) { fclose(f); if (g) luxb_close(g); return rc; }
   g->nv = nv;
   g->ne = ne;
-  g->weighted = cfg->app == LUXB_COLFILTER;
+  g->weighted = uses_weights(cfg->app);
   g->parts_found = host_partition(nv, ne, row_end.data(), g->P, g->ref_rl, g->ref_np, g->ref_cl);
   if (use_balanced_split(cfg)) host_balanced_partition(nv, ne, row_end.data(), g->P, g->rl, g->np, g->cl);
   else for (int p = 0; p < g->P; ++p) { g->rl[p] = g->ref_rl[p]; g->np[p] = g->ref_np[p]; g->cl[p] = g->ref_cl[p]; }
@@ -464,7 +478,7 @@ static int open_generated(const GenSpec& spec, const luxb_config* cfg, luxb_grap
   auto fail = [&](int code) { luxb_close(g); return code; };
   g->nv = spec.nv;
   g->ne = spec.ne;
-  g->weighted = cfg->app == LUXB_COLFILTER;
+  g->weighted = uses_weights(cfg->app);
   const int gen_grid = g->num_sms * 16;
   // 1. in-degree histogram over the whole edge stream -> global row_end (u64) by an inclusive scan
   uint32_t* d_indeg = nullptr;
@@ -557,7 +571,11 @@ static int open_generated(const GenSpec& spec, const luxb_config* cfg, luxb_grap
     if ((rc = edge_alloc(g, &g->d_weight, g->e_part + 8))) return fail(rc);
     GEN_CUDA(cudaMemsetAsync(g->d_weight, 0, (g->e_part + 8) * 4, g->stream));
   }
-  keys_to_src_kernel<<<gen_grid, 256, 0, g->stream>>>(keys.Current(), g->e_part, g->d_src, g->d_weight, spec.seed, g->row_left);
+  // bipartite: the ratings 1..5 of the (user, item) pair; RMAT (weighted SSSP): directed weights 1..255
+  keys_to_src_kernel<<<gen_grid, 256, 0, g->stream>>>(keys.Current(), g->e_part, g->d_src, spec.kind == 0 ? nullptr : g->d_weight,
+                                                      spec.seed, g->row_left);
+  if (spec.kind == 0 && g->weighted)
+    keys_to_rmat_weight_kernel<<<gen_grid, 256, 0, g->stream>>>(keys.Current(), g->e_part, g->d_weight, spec.seed, g->row_left);
   GEN_CUDA(cudaGetLastError());
   GEN_CUDA(cudaStreamSynchronize(g->stream));
   GEN_CUDA(cudaFree(d_keys));
@@ -843,6 +861,21 @@ static int build_push_csr(luxb_graph* g) {
   LUXB_TRY(tmp.alloc((char**)&d_tmp, tmp_bytes + 256));
   LUXB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, g->d_src, d_keys_out, d_dst, g->d_out_dst, (long long)g->e_part, 0,
                                             vbits, g->stream));
+  if (g->cfg.app == LUXB_SSSP_WEIGHTED) {
+    // the weights in the same order: the same stable sort on the same keys applies the same permutation
+    LUXB_TRY(dmalloc(&g->d_out_w, g->e_part));
+    size_t w_bytes = 0;
+    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, w_bytes, g->d_src, d_keys_out, g->d_weight, g->d_out_w, (long long)g->e_part, 0,
+                                              vbits, g->stream));
+    if (w_bytes > tmp_bytes) {
+      LUXB_CUDA(cudaStreamSynchronize(g->stream));
+      tmp.release(d_tmp);
+      LUXB_TRY(tmp.alloc((char**)&d_tmp, w_bytes + 256));
+      tmp_bytes = w_bytes;
+    }
+    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, g->d_src, d_keys_out, g->d_weight, g->d_out_w, (long long)g->e_part, 0,
+                                              vbits, g->stream));
+  }
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
   return 0;
 }
@@ -881,7 +914,8 @@ static int reset_label_state(luxb_graph* g, bool all_active) {
     const int grid = g->num_sms * 8;
     if (cc) iota_kernel<<<grid, 256, 0, g->stream>>>(lab, g->nv);
     else {
-      fill_kernel<uint32_t><<<grid, 256, 0, g->stream>>>(lab, g->nv, g->nv);
+      // INF: nv for hop counts (sssp_gpu.cu:733-744), LUXB_DIST_INF for weighted distances
+      fill_kernel<uint32_t><<<grid, 256, 0, g->stream>>>(lab, g->nv, g->cfg.app == LUXB_SSSP_WEIGHTED ? kDistInf : g->nv);
       uint32_t zero = 0;
       if (g->cfg.start_vtx < g->nv)
         LUXB_CUDA(cudaMemcpyAsync(lab + g->cfg.start_vtx, &zero, 4, cudaMemcpyHostToDevice, g->stream));
@@ -1154,9 +1188,10 @@ int luxb_init(luxb_graph* g) {
       break;
     }
     case LUXB_CC:
-    case LUXB_SSSP: {
+    case LUXB_SSSP:
+    case LUXB_SSSP_WEIGHTED: {
       g->vbytes = 4;
-      LUXB_ARG(g->cfg.app != LUXB_SSSP || g->cfg.start_vtx < g->nv, "start vertex %u >= nv", g->cfg.start_vtx);
+      LUXB_ARG(g->cfg.app == LUXB_CC || g->cfg.start_vtx < g->nv, "start vertex %u >= nv", g->cfg.start_vtx);
       LUXB_TRY(dmalloc((uint32_t**)&g->d_val[0], g->nv));
       LUXB_TRY(dmalloc(&g->d_cur, g->n_part));
       LUXB_TRY(build_push_csr(g));
@@ -1167,7 +1202,8 @@ int luxb_init(luxb_graph* g) {
         LUXB_CUDA(cudaGetLastError());
         if (g->P > 1) LUXB_NCCL(nccl().AllReduce(g->d_deg, g->d_deg, g->nv, ncclUint32, ncclSum, g->comm, g->stream));
         LUXB_TRY(build_hot_layout(g, /*compact_cold=*/false));
-        LUXB_TRY(build_seg_sweep(g));
+        // weighted SSSP pulls through the merge-path sweep only: the flagged streams carry no weights
+        if (g->cfg.app != LUXB_SSSP_WEIGHTED) LUXB_TRY(build_seg_sweep(g));
         if (g->hot_n) {
           LUXB_TRY(dmalloc((uint32_t**)&g->d_hot, (uint64_t)g->hot_n + 65536));  // + one table of slack (panel.cuh)
           LUXB_CUDA(cudaMemsetAsync(g->d_hot, 0, ((size_t)g->hot_n + 65536) * 4, g->stream));
@@ -1263,14 +1299,15 @@ template <class Prog, class Shape>
 static int launch_pull_shape(luxb_graph* g, const PullArgs<Prog>& a) {
   auto kern = pull_tile_kernel<Prog, Shape>;
   const int want = g->pull_ctas;
+  constexpr size_t smem = pull_smem_bytes<Prog, Shape>();
   // carve out exactly `want` CTAs' worth of shared memory; the rest of the 256 KB unified array stays L1.
   // (function attributes are per device and idempotent: set on every launch, no process-global cache)
-  LUXB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Shape::kSmemBytes));
-  int carve_pct = (int)std::min<size_t>(100, (want * (Shape::kSmemBytes + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024));
+  LUXB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int carve_pct = (int)std::min<size_t>(100, (want * (smem + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024));
   LUXB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, carve_pct));
   const uint32_t n_super = (a.n_tiles + Shape::kWarps - 1) / Shape::kWarps;
   uint32_t grid = (uint32_t)std::min<uint64_t>((uint64_t)g->num_sms * want, n_super);
-  kern<<<grid, Shape::kThreads, Shape::kSmemBytes, g->stream>>>(a);
+  kern<<<grid, Shape::kThreads, smem, g->stream>>>(a);
   LUXB_CUDA(cudaGetLastError());
   return 0;
 }
@@ -1363,6 +1400,7 @@ static int launch_pull(luxb_graph* g, PullLayout& L, const typename Prog::Vertex
   a.prm = prm;
   a.hub_bits = hub_bits;
   a.raw_out = 0;
+  if constexpr (Prog::kWeighted) a.weight = g->d_weight;  // CSC order = the order of L.d_src (base layout only)
   if (timed) LUXB_TRY(kt_begin(g));
   switch (g->pull_shape) {
 #define LUXB_CASE_SHAPE(id, ipt, warps, stages) \
@@ -2140,12 +2178,16 @@ static int label_iteration(luxb_graph* g) {
       hot_refresh_kernel<uint32_t><<<grid_for(g->hot_n, 256, g->num_sms * 8), 256, 0, g->stream>>>((uint32_t*)g->d_hot, lab, g->d_hot_order, 0, g->hot_n);
       g->stats.kernel_launches++;
     }
-    if (g->seg_on) {
-      LUXB_TRY((sweep_seg<Prog>(g, lab, lab, g->d_cur, -1, prm)));
-    } else {
+    bool swept = false;
+    if constexpr (!Prog::kWeighted) {  // weighted programs never build the flagged streams (no weights there)
+      if (g->seg_on) {
+        LUXB_TRY((sweep_seg<Prog>(g, lab, lab, g->d_cur, -1, prm)));
+        swept = true;
+      }
+    }
+    if (!swept)
       LUXB_TRY(launch_pull<Prog>(g, base_layout(g, g->hot_n ? g->d_src_gather : g->d_src), lab, lab, (const uint32_t*)g->d_hot, g->hot_n,
                                  g->d_cur, prm));
-    }
     g->stats.edges_processed += g->e_part;
     g->stats.pull_iterations++;
   } else if (g->n_part && old_size) {
@@ -2175,6 +2217,7 @@ static int label_iteration(luxb_graph* g) {
     a.big_list = reinterpret_cast<PushArgs::BigSeg*>(g->d_big_list);
     a.big_count = reinterpret_cast<uint32_t*>(g->d_counters + 3);
     a.big_capacity = g->big_capacity;
+    a.out_w = g->d_out_w;
     if (blocks) {
       LUXB_CUDA(cudaMemsetAsync(a.big_count, 0, 4, g->stream));
       push_relax_kernel<Prog><<<(unsigned)blocks, kPushThreads, 0, g->stream>>>(a);
@@ -2344,6 +2387,7 @@ static int one_iteration(luxb_graph* g) {
     case LUXB_COLFILTER: return colfilter_iteration(g);
     case LUXB_CC: return label_iteration<MaxLabelProgram>(g);
     case LUXB_SSSP: return label_iteration<HopDistProgram>(g);
+    case LUXB_SSSP_WEIGHTED: return label_iteration<WeightedDistProgram>(g);
   }
   return LUXB_ERR_ARG;
 }
@@ -2401,7 +2445,7 @@ int luxb_iterate(luxb_graph* g, int iters, uint64_t* active_out) {
 int luxb_run_to_convergence(luxb_graph* g, int max_iters, int* iters_out) {
   LUXB_ARG(g != nullptr, "graph is NULL");
   if (!g->inited) { set_error("luxb_run_to_convergence before luxb_init"); return LUXB_ERR_STATE; }
-  LUXB_ARG(g->cfg.app == LUXB_CC || g->cfg.app == LUXB_SSSP, "only push apps converge (pagerank/col_filter run -ni iterations)");
+  LUXB_ARG(is_label_app(g->cfg.app), "only push apps converge (pagerank/col_filter run -ni iterations)");
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
   LUXB_CUDA(cudaEventRecord(g->ev_begin, g->stream));
   int it = 0;
@@ -2433,7 +2477,7 @@ int luxb_get_values(luxb_graph* g, void* host_out, size_t bytes) {
   LUXB_ARG(bytes == need, "buffer is %zu bytes, vertex values need %zu", bytes, need);
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
   LUXB_TRY(refresh_replica(g));
-  const char* srcp = (const char*)((g->cfg.app == LUXB_CC || g->cfg.app == LUXB_SSSP) ? g->d_val[0] : g->d_val[g->cur]);
+  const char* srcp = (const char*)(is_label_app(g->cfg.app) ? g->d_val[0] : g->d_val[g->cur]);
   LUXB_CUDA(cudaMemcpyAsync(host_out, srcp, need, cudaMemcpyDeviceToHost, g->stream));
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
   return 0;
@@ -2445,7 +2489,7 @@ int luxb_get_local_values(luxb_graph* g, void* host_out, size_t bytes) {
   size_t need = (size_t)g->n_part * g->vbytes;
   LUXB_ARG(bytes == need, "buffer is %zu bytes, this rank's %u vertex values need %zu", bytes, g->n_part, need);
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
-  const char* base = (const char*)((g->cfg.app == LUXB_CC || g->cfg.app == LUXB_SSSP) ? g->d_val[0] : g->d_val[g->cur]);
+  const char* base = (const char*)(is_label_app(g->cfg.app) ? g->d_val[0] : g->d_val[g->cur]);
   if (need) LUXB_CUDA(cudaMemcpyAsync(host_out, base + (size_t)g->row_left * g->vbytes, need, cudaMemcpyDeviceToHost, g->stream));
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
   return 0;
@@ -2454,7 +2498,7 @@ int luxb_get_local_values(luxb_graph* g, void* host_out, size_t bytes) {
 // values of the vertices are in place in the current replica (whole array, or only this rank's slice): make them the
 // state the next iteration starts from on every rank
 static int values_installed(luxb_graph* g, bool whole_array) {
-  const bool labels = g->cfg.app == LUXB_CC || g->cfg.app == LUXB_SSSP;
+  const bool labels = is_label_app(g->cfg.app);
   if (g->cfg.app == LUXB_PAGERANK) {
     g->empties_done[g->cur] = false;  // caller data now sits where the constants of the edge-less vertices were
     LUXB_TRY(pagerank_publish(g, (float*)g->d_val[g->cur]));
@@ -2473,7 +2517,7 @@ int luxb_set_values(luxb_graph* g, const void* host_in, size_t bytes) {
   size_t need = (size_t)g->nv * g->vbytes;
   LUXB_ARG(bytes == need, "buffer is %zu bytes, vertex values need %zu", bytes, need);
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
-  const bool labels = g->cfg.app == LUXB_CC || g->cfg.app == LUXB_SSSP;
+  const bool labels = is_label_app(g->cfg.app);
   char* dstp = (char*)(labels ? g->d_val[0] : g->d_val[g->cur]);
   LUXB_CUDA(cudaMemcpyAsync(dstp, host_in, need, cudaMemcpyHostToDevice, g->stream));
   return values_installed(g, true);
@@ -2485,7 +2529,7 @@ int luxb_set_local_values(luxb_graph* g, const void* host_in, size_t bytes) {
   size_t need = (size_t)g->n_part * g->vbytes;
   LUXB_ARG(bytes == need, "buffer is %zu bytes, this rank's %u vertex values need %zu", bytes, g->n_part, need);
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
-  const bool labels = g->cfg.app == LUXB_CC || g->cfg.app == LUXB_SSSP;
+  const bool labels = is_label_app(g->cfg.app);
   char* dstp = (char*)(labels ? g->d_val[0] : g->d_val[g->cur]);
   if (need) LUXB_CUDA(cudaMemcpyAsync(dstp + (size_t)g->row_left * g->vbytes, host_in, need, cudaMemcpyHostToDevice, g->stream));
   return values_installed(g, false);
@@ -2494,7 +2538,7 @@ int luxb_set_local_values(luxb_graph* g, const void* host_in, size_t bytes) {
 int luxb_check(luxb_graph* g, uint64_t* mistakes_out) {
   LUXB_ARG(g && mistakes_out, "NULL argument");
   if (!g->inited) { set_error("luxb_check before luxb_init"); return LUXB_ERR_STATE; }
-  LUXB_ARG(g->cfg.app == LUXB_CC || g->cfg.app == LUXB_SSSP,
+  LUXB_ARG(is_label_app(g->cfg.app),
            "the reference has no check for pagerank / col_filter (CHECK_TASK_ID is not registered in pull_model.inl:482-521)");
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
   LUXB_CUDA(cudaMemsetAsync(g->d_counters + 1, 0, 8, g->stream));
@@ -2503,8 +2547,11 @@ int luxb_check(luxb_graph* g, uint64_t* mistakes_out) {
   if (g->n_part) {
     if (g->cfg.app == LUXB_CC)
       check_kernel<MaxLabelProgram><<<grid, 256, 0, g->stream>>>(g->d_row_end, g->d_src, g->n_part, g->row_left, g->nv, lab, g->d_counters + 1);
-    else
+    else if (g->cfg.app == LUXB_SSSP)
       check_kernel<HopDistProgram><<<grid, 256, 0, g->stream>>>(g->d_row_end, g->d_src, g->n_part, g->row_left, g->nv, lab, g->d_counters + 1);
+    else
+      check_kernel<WeightedDistProgram><<<grid, 256, 0, g->stream>>>(g->d_row_end, g->d_src, g->n_part, g->row_left, lab, g->d_counters + 1,
+                                                                     g->d_weight);
     LUXB_CUDA(cudaGetLastError());
   }
   unsigned long long bad = 0;
@@ -2587,7 +2634,7 @@ int luxb_debug_gather_ms(luxb_graph* g, int packed, float* ms_out) {
 
 int luxb_device_view_get(luxb_graph* g, luxb_device_view* out) {
   LUXB_ARG(g && out, "NULL argument");
-  const bool labels = g->cfg.app == LUXB_CC || g->cfg.app == LUXB_SSSP;
+  const bool labels = is_label_app(g->cfg.app);
   out->values = g->inited ? (labels ? g->d_val[0] : g->d_val[g->cur]) : nullptr;
   out->row_end = g->d_row_end;
   out->src = g->d_src;
@@ -2628,7 +2675,7 @@ void luxb_close(luxb_graph* g) {
   if (g->stream2) cudaStreamDestroy(g->stream2);
 
   void* ptrs[] = {g->d_row_end, g->d_row_end32, g->d_src, g->d_weight, g->d_tile_v, g->d_head, g->d_tail, g->d_deg, g->d_val[0], g->d_val[1],
-                  g->d_cur, g->d_out_end, g->d_out_dst, g->d_fq_all, g->d_fq_new, g->d_fq_tmp, g->d_hdr_all, g->d_counters,
+                  g->d_cur, g->d_out_end, g->d_out_dst, g->d_out_w, g->d_fq_all, g->d_fq_new, g->d_fq_tmp, g->d_hdr_all, g->d_counters,
                   g->d_chunk_first, g->d_chunk_vtx, g->d_partial, g->d_sync, g->d_hot_order, g->d_src_gather,
                   g->d_carry, g->d_carry_flag, g->d_block_agg, g->d_block_flag, g->d_hot, g->d_big_list};
   for (void* p : ptrs) {

@@ -42,6 +42,13 @@ __device__ __forceinline__ int32_t edge_weight(uint64_t seed, uint32_t src, uint
   return (int32_t)(1 + (h >> 33) % 5);
 }
 
+// weighted SSSP on RMAT: a directed weight in [1, 255] that depends only on (seed, src, dst); MUST match
+// tests/weighted_oracle.c wo_rmat_weight bit for bit
+__device__ __forceinline__ int32_t rmat_weight(uint64_t seed, uint32_t src, uint32_t dst) {
+  uint64_t h = splitmix64(splitmix64(seed ^ 0x9E3779B97F4A7C15ull) ^ (((uint64_t)dst << 32) | src));
+  return (int32_t)(1 + (h >> 32) % 255);
+}
+
 __device__ __forceinline__ void bipartite_edge(uint64_t seed_mixed, uint64_t j, uint32_t users, uint32_t items,
                                                uint32_t& user, uint32_t& item) {
   uint64_t h1 = splitmix64(seed_mixed ^ j);
@@ -122,6 +129,15 @@ __global__ void keys_to_src_kernel(const uint64_t* __restrict__ keys, uint64_t n
       uint32_t lo = s < d ? s : d, hi = s < d ? d : s;
       weight[e] = edge_weight(seed, lo, hi);
     }
+  }
+}
+
+// RMAT weights of the sorted keys ((dst - row_left) << 32 | src), in CSC order
+__global__ void keys_to_rmat_weight_kernel(const uint64_t* __restrict__ keys, uint64_t n, int32_t* __restrict__ weight, uint64_t seed,
+                                           uint32_t row_left) {
+  for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (uint64_t)gridDim.x * blockDim.x) {
+    uint64_t k = keys[e];
+    weight[e] = rmat_weight(seed, (uint32_t)k, (uint32_t)(k >> 32) + row_left);
   }
 }
 
@@ -208,6 +224,13 @@ __global__ void rowend_rel_kernel(const uint64_t* __restrict__ row_end_global, u
 __global__ void src_out_of_range_kernel(const uint32_t* __restrict__ src, uint64_t n, uint32_t nv, unsigned long long* __restrict__ bad) {
   unsigned long long c = 0;
   for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (uint64_t)gridDim.x * blockDim.x) c += src[e] >= nv;
+  if (c) atomicAdd(bad, c);
+}
+
+// number of negative weights in this rank's slice (weighted SSSP needs w >= 0)
+__global__ void negative_weight_kernel(const int32_t* __restrict__ w, uint64_t n, unsigned long long* __restrict__ bad) {
+  unsigned long long c = 0;
+  for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (uint64_t)gridDim.x * blockDim.x) c += w[e] < 0;
   if (c) atomicAdd(bad, c);
 }
 

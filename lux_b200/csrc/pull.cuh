@@ -15,6 +15,8 @@
 //      pair per stage — measured: ~1 small bulk copy per 400 cycles per SM, so one copy pair serves 8 warp tiles
 //      (~7 KB) instead of one (per-warp copies made the kernel 2-4x slower).  L2 evict-first: streamed data must not displace the value array.  Consumer warps only
 //      meet at these mbarriers and may drift kStages-1 super-tiles apart;
+//      Weighted programs (weighted SSSP) add a third bulk copy per super-tile: the edge weights of the same range into
+//      a weight ring next to the source-id ring;
 //   2. every lane finds its merge-path start by binary search over <= W row_end words in shared memory, then issues
 //      its (up to kIPT) gathers x[src] back to back on the read-only path — values land in REGISTERS in the order
 //      the lane will consume them (no shared-memory round trip);
@@ -45,10 +47,26 @@ struct PullShape {
   static constexpr size_t kSmemBytes = (size_t)kStages * (kAElems + kEElems) * 4 + (size_t)kWarps * kSumElems * 4 +
                                        2 * kStages * 8 + (size_t)kStages * kHdrElems * 4 + 16;
   static_assert(kIPT % 2 == 1, "kIPT must be odd: lane-contiguous smem reads are then bank-conflict free");
+  static constexpr size_t kWRingOffset = (kSmemBytes + 15) & ~(size_t)15;  // weighted programs: weight ring after the rest
+};
+
+// dynamic shared memory of pull_tile_kernel<Prog, Shape>: weighted programs add a ring of kStages x kEElems weights
+template <class Prog, class Shape>
+constexpr size_t pull_smem_bytes() {
+  return Prog::kWeighted ? Shape::kWRingOffset + (size_t)Shape::kStages * Shape::kEElems * 4 : Shape::kSmemBytes;
+}
+
+// weighted programs: [ePart + 8] i32 edge weights in CSC edge order (the same positions as src).  An empty base for the
+// others, so that their PullArgs (and the SegArgs holding one) keep their layout byte for byte.
+template <bool kWeighted>
+struct PullWeights {};
+template <>
+struct PullWeights<true> {
+  const int32_t* weight;
 };
 
 template <class Prog>
-struct PullArgs {
+struct PullArgs : PullWeights<Prog::kWeighted> {
   const uint64_t* row_end;   // [nPart + 4] end offsets relative to the partition's first edge; padded with ~0
   const uint32_t* row_end32; // [nPart + 8] low 32 bits of row_end: what the tile kernel streams (differences inside
                              // a tile are < 2^32, so tile-relative offsets are exact modulo 2^32)
@@ -215,9 +233,20 @@ __global__ void __launch_bounds__(Shape::kThreads) pull_tile_kernel(const __grid
         const uint64_t js = j0 & ~3ull;
         uint32_t bytes_e = (uint32_t)(((j1 - js) * 4 + 15) & ~15ull);
         if (j1 == j0) bytes_e = 0;
-        mbar_arrive_expect_tx(&full[s], bytes_a + bytes_e);
-        bulk_g2s(a_buf + (size_t)s * Shape::kAElems, a.row_end32 + is, bytes_a, &full[s], policy);
-        if (bytes_e) bulk_g2s(e_buf + (size_t)s * Shape::kEElems, a.src + js, bytes_e, &full[s], policy);
+        if constexpr (Prog::kWeighted) {
+          // third copy: the weights of the same edge range, into the weight ring
+          mbar_arrive_expect_tx(&full[s], bytes_a + 2 * bytes_e);
+          bulk_g2s(a_buf + (size_t)s * Shape::kAElems, a.row_end32 + is, bytes_a, &full[s], policy);
+          if (bytes_e) {
+            bulk_g2s(e_buf + (size_t)s * Shape::kEElems, a.src + js, bytes_e, &full[s], policy);
+            int32_t* w_buf = reinterpret_cast<int32_t*>(smem_raw + Shape::kWRingOffset);
+            bulk_g2s(w_buf + (size_t)s * Shape::kEElems, a.weight + js, bytes_e, &full[s], policy);
+          }
+        } else {
+          mbar_arrive_expect_tx(&full[s], bytes_a + bytes_e);
+          bulk_g2s(a_buf + (size_t)s * Shape::kAElems, a.row_end32 + is, bytes_a, &full[s], policy);
+          if (bytes_e) bulk_g2s(e_buf + (size_t)s * Shape::kEElems, a.src + js, bytes_e, &full[s], policy);
+        }
       }
       __syncwarp();
     }
@@ -269,7 +298,13 @@ __global__ void __launch_bounds__(Shape::kThreads) pull_tile_kernel(const __grid
           const uint32_t id = E[j + k];
           const bool hot = id < a.hot_n;
           const Vertex* p = hot ? a.x_hot + id : a.x_old + (id - a.hot_n);
-          val[k] = Prog::gather(gather_load(p, hot));
+          if constexpr (Prog::kWeighted) {
+            const int32_t* W = reinterpret_cast<const int32_t*>(smem_raw + Shape::kWRingOffset) + (size_t)s * Shape::kEElems +
+                               (uint32_t)(sj0 & 3ull) + (uint32_t)(j0 - sj0);  // the weights at E's positions
+            val[k] = Prog::gather(gather_load(p, hot), W[j + k]);
+          } else {
+            val[k] = Prog::gather(gather_load(p, hot));
+          }
         }
 
       // ---- serial walk: edges [j, j_next) merged with vertex-end markers [i, i_next) ----

@@ -50,6 +50,9 @@ struct PushArgs {
   BigSeg* big_list;
   uint32_t* big_count;
   uint32_t big_capacity;
+  // weighted programs: [ePart] i32 weight of each out-edge, aligned with out_dst.  s_val / BigSeg::val then carry the
+  // source's raw label and every edge adds its own weight
+  const int32_t* out_w;
 };
 
 constexpr uint32_t kPushBigDegree = 2048;
@@ -130,7 +133,8 @@ __global__ void __launch_bounds__(kPushThreads) push_relax_kernel(const __grid_c
       uint64_t e1 = a.out_end[u];
       begin = u == 0 ? 0 : a.out_end[u - 1];
       deg = e1 - begin;
-      val = Prog::gather(a.lab[u]);
+      if constexpr (Prog::kWeighted) val = a.lab[u];
+      else val = Prog::gather(a.lab[u]);
       if (deg > kPushBigDegree) {
         uint32_t n_seg = (uint32_t)((deg + kPushSegment - 1) / kPushSegment);
         uint32_t pos = atomicAdd(a.big_count, n_seg);
@@ -176,8 +180,10 @@ __global__ void __launch_bounds__(kPushThreads) push_relax_kernel(const __grid_c
         int mid = (lo + hi) >> 1;
         if (s_scan[mid] <= e) lo = mid; else hi = mid;
       }
-      dstv = a.out_dst[s_begin[lo] + (e - s_scan[lo])];
-      enq = relax_edge<Prog>(a, dstv, s_val[lo]);
+      const uint64_t k = s_begin[lo] + (e - s_scan[lo]);
+      dstv = a.out_dst[k];
+      if constexpr (Prog::kWeighted) enq = relax_edge<Prog>(a, dstv, Prog::gather(s_val[lo], a.out_w[k]));
+      else enq = relax_edge<Prog>(a, dstv, s_val[lo]);
     }
     enqueue_warp(a, enq, dstv, lane);
   }
@@ -198,7 +204,8 @@ __global__ void __launch_bounds__(kPushThreads) push_big_kernel(const __grid_con
       uint32_t dstv = 0;
       if (e < sg.len) {
         dstv = a.out_dst[sg.begin + e];
-        enq = relax_edge<Prog>(a, dstv, sg.val);
+        if constexpr (Prog::kWeighted) enq = relax_edge<Prog>(a, dstv, Prog::gather(sg.val, a.out_w[sg.begin + e]));
+        else enq = relax_edge<Prog>(a, dstv, sg.val);
       }
       enqueue_warp(a, enq, dstv, lane);
     }
@@ -414,6 +421,24 @@ __global__ void check_kernel(const uint64_t* __restrict__ row_end_rel, const uin
     for (uint64_t k = b; k < e; ++k) {
       uint32_t ls = lab[src[k]];
       if (Prog::kIsMax) bad += ld < ls; else bad += (ls != nv) && (ld > ls + 1);
+    }
+  }
+  if (bad) atomicAdd(mistakes, bad);
+}
+
+// weighted SSSP: D[u] != INF  =>  D[v] <= sat_add(D[u], w(u,v)), over this partition's in-edges and their CSC weights
+template <class Prog>
+__global__ void check_kernel(const uint64_t* __restrict__ row_end_rel, const uint32_t* __restrict__ src, uint32_t n_part,
+                             uint32_t row_left, const uint32_t* __restrict__ lab, unsigned long long* __restrict__ mistakes,
+                             const int32_t* __restrict__ weight) {
+  static_assert(Prog::kWeighted, "the weighted predicate");
+  unsigned long long bad = 0;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_part; i += (uint64_t)gridDim.x * blockDim.x) {
+    uint64_t b = i == 0 ? 0 : row_end_rel[i - 1], e = row_end_rel[i];
+    uint32_t ld = lab[row_left + i];
+    for (uint64_t k = b; k < e; ++k) {
+      uint32_t ls = lab[src[k]];
+      bad += (ls != kDistInf) && (ld > Prog::gather(ls, weight[k]));
     }
   }
   if (bad) atomicAdd(mistakes, bad);

@@ -121,6 +121,7 @@ struct luxb_graph {
   uint32_t* d_cur = nullptr;       // [n_part] working labels of this partition
   uint64_t* d_out_end = nullptr;   // [nv] CSR-by-source end offsets over this partition's edges
   uint32_t* d_out_dst = nullptr;   // [e_part]
+  int32_t* d_out_w = nullptr;      // [e_part] weighted SSSP: the weight of each out-edge, aligned with d_out_dst
   void* d_big_list = nullptr;      // segments of hub sources' out-edge lists (push_big_kernel)
   uint32_t big_capacity = 0;
   unsigned char* d_fq_all = nullptr;  // every partition's frontier slot as exchanged
