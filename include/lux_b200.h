@@ -211,6 +211,9 @@ typedef struct {
   uint32_t panel_blocks;     /*   hot source blocks */
   uint64_t cold_hub_edges;   /* PageRank, one rank: local (cold source -> hub) edges swept by segment of the cold values */
   uint32_t cold_hub_segments; /*   cold source segments (0 = no cold-hub stream) */
+  uint32_t tier_blocks;      /* PageRank: hot source blocks after the first panel_blocks, each over a prefix of the hubs */
+  uint64_t tier_slots;       /*   their (block, hub) slots */
+  uint64_t tier_edges;       /*   their edges */
 } luxb_stats_t;
 int luxb_stats(const luxb_graph* g, luxb_stats_t* out);
 /* Per-iteration trace of push apps (global active count, direction) for parity tests; returns #entries copied. */

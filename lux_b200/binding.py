@@ -38,7 +38,8 @@ class Stats(C.Structure):
                 ("pull_iterations", C.c_uint64), ("kernel_launches", C.c_uint64), ("last_active", C.c_uint64),
                 ("last_frontier_type", C.c_uint32), ("dominant_kernel_seconds", C.c_double),
                 ("dominant_kernel_launches", C.c_uint64), ("panel_edges", C.c_uint64), ("panel_hubs", C.c_uint32),
-                ("panel_blocks", C.c_uint32), ("cold_hub_edges", C.c_uint64), ("cold_hub_segments", C.c_uint32)]
+                ("panel_blocks", C.c_uint32), ("cold_hub_edges", C.c_uint64), ("cold_hub_segments", C.c_uint32),
+                ("tier_blocks", C.c_uint32), ("tier_slots", C.c_uint64), ("tier_edges", C.c_uint64)]
 
 
 class DeviceView(C.Structure):

@@ -959,6 +959,8 @@ static int set_l2_persisting_window(luxb_graph* g, void* base, size_t bytes) {
 
 // cold -> hub edges (PageRank, one rank) get a stream of their own when they are at least this share of the partition
 static constexpr double kColdSplitMinShare = 0.05;
+// panel tiers (build_panel_layout): a (block, hub) slot past tier 0 is kept when it expects at least this many edges
+static constexpr double kTierSlotEdges = 0.5;
 
 // Choose the hot set (largest out-degrees, at most LUXB_HOT_MB megabytes of values, default 24 MB ~ half of the H100's
 // 50 MB L2: at RMAT-27 on one H100 8 / 16 / 24 / 32 / 64 MB gave 21.4 / 15.8 / 14.2 / 16.7 / 17.3 ms per sweep) and
@@ -1570,7 +1572,10 @@ static int build_plain_seg_layout(luxb_graph* g) {
 // Split this partition's (hot-packed) CSC into the panel (hot source block x hub destination, 15-bit offsets, gathered
 // from shared memory) and the main stream (everything else, gathered through L1).
 // LUXB_SB = 0 off / 1 force / unset: automatic (on when the panel would take at least a fifth of a large partition).
-// Tuning: LUXB_SB_BS (values per block), LUXB_SB_BLOCKS (max blocks), LUXB_SB_MIN_INDEG (hub threshold).
+// Tuning: LUXB_SB_BS (values per block), LUXB_SB_BLOCKS (tier 0: max blocks over all hubs), LUXB_SB_MIN_INDEG (hub
+// threshold).  Tiers (panel.cuh): the blocks after tier 0 cover the rest of the hot set, block b over the hubs of
+// in-degree d with d * m_b >= LUXB_SB_SLOT_EDGES (expected edges per slot; m_b = block b's share of the hubs' in-edges).
+// LUXB_SB_TIER = 0 off / 1 force / unset: on where the cold-hub stream may be (one rank) on a partition of >= 2^24 edges.
 // With the compact cold values of one rank (cold_z), the cold -> hub edges form a third stream (panel.cuh, ColdSplit):
 // LUXB_CS = 0 off / 1 force / unset: on when they are at least kColdSplitMinShare of the partition's edges;
 // LUXB_CS_SEG_MB: segment size (raised where the segments would not fit the sort key), LUXB_CS_SHAPE: its main shape.
@@ -1584,8 +1589,11 @@ static int build_panel_layout(luxb_graph* g) {
   uint32_t bs = (uint32_t)std::max(4, env_int("LUXB_SB_BS", shp.tab));
   bs = std::min<uint32_t>(bs & ~3u, (uint32_t)shp.tab);
   const uint32_t nb_max = (uint32_t)std::min(std::max(env_int("LUXB_SB_BLOCKS", 48), 1), kPanelMaxBlocks);
-  const uint32_t n_src = (uint32_t)std::min<uint64_t>(g->hot_n, (uint64_t)nb_max * bs);
-  const uint32_t NB = (n_src + bs - 1) / bs;
+  const uint32_t NB0 = (uint32_t)((std::min<uint64_t>(g->hot_n, (uint64_t)nb_max * bs) + bs - 1) / bs);  // tier 0
+  const int tier_mode = env_int("LUXB_SB_TIER", -1);
+  const bool tiers = tier_mode > 0 || (tier_mode < 0 && g->cold_z && g->e_part >= (1ull << 24));
+  const uint32_t nb_all = tiers ? (uint32_t)std::min<uint64_t>(((uint64_t)g->hot_n + bs - 1) / bs, kPanelMaxBlocks) : NB0;
+  const double slot_edges = [] { const char* e = getenv("LUXB_SB_SLOT_EDGES"); return e ? atof(e) : kTierSlotEdges; }();
   const uint32_t min_indeg = (uint32_t)std::max(env_int("LUXB_SB_MIN_INDEG", 64), 1);
   const int grid = g->num_sms * 8;
   DevTmp tmp;
@@ -1607,15 +1615,45 @@ static int build_panel_layout(luxb_graph* g) {
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
   tmp.release(d_scan_tmp);
   const uint32_t Nh = last_idx + last_flag;
-  if (Nh == 0 || (uint64_t)Nh * NB >= 0x7FFFFFF0ull) return 0;
+  if (Nh == 0 || (uint64_t)Nh * NB0 >= 0x7FFFFFF0ull) return 0;
   uint32_t *d_hub_vtx = nullptr, *d_hub_bits = nullptr, *d_cov = nullptr;
   LUXB_TRY(tmp.alloc(&d_hub_vtx, Nh));
   LUXB_TRY(tmp.alloc(&d_hub_bits, ((uint64_t)g->n_part + 31) / 32 + 1));
   LUXB_TRY(tmp.alloc(&d_cov, Nh));
   hub_list_kernel<<<grid, 256, 0, g->stream>>>(d_flag, d_hub_idx, g->n_part, d_hub_vtx, d_hub_bits);
   LUXB_CUDA(cudaGetLastError());
+  // hubs by in-degree, descending: the hub prefix of every block holds the hubs of highest in-degree
+  std::vector<uint32_t> hub_key(Nh);  // ~in-degree, ascending
+  {
+    uint32_t *d_hkey = nullptr, *d_hkey2 = nullptr, *d_hvtx2 = nullptr;
+    LUXB_TRY(tmp.alloc(&d_hkey, Nh));
+    LUXB_TRY(tmp.alloc(&d_hkey2, Nh));
+    LUXB_TRY(tmp.alloc(&d_hvtx2, Nh));
+    hub_order_key_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, d_hub_vtx, Nh, d_hkey);
+    LUXB_CUDA(cudaGetLastError());
+    tb = 0;
+    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_hkey, d_hkey2, d_hub_vtx, d_hvtx2, (int)Nh, 0, 32, g->stream));
+    LUXB_TRY(tmp.alloc((char**)&d_scan_tmp, tb + 256));
+    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(d_scan_tmp, tb, d_hkey, d_hkey2, d_hub_vtx, d_hvtx2, (int)Nh, 0, 32, g->stream));
+    LUXB_CUDA(cudaMemcpyAsync(d_hub_vtx, d_hvtx2, (size_t)Nh * 4, cudaMemcpyDeviceToDevice, g->stream));
+    hub_pos_kernel<<<grid, 256, 0, g->stream>>>(d_hub_vtx, Nh, d_hub_idx);
+    LUXB_CUDA(cudaGetLastError());
+    LUXB_CUDA(cudaMemcpyAsync(hub_key.data(), d_hkey2, (size_t)Nh * 4, cudaMemcpyDeviceToHost, g->stream));
+    LUXB_CUDA(cudaStreamSynchronize(g->stream));
+    tmp.release(d_scan_tmp);
+    tmp.release(d_hkey);
+    tmp.release(d_hkey2);
+    tmp.release(d_hvtx2);
+  }
+  // hub prefix N_b of every block: all hubs for now (tier 0 keeps them; the tiers are decided from the first keying)
+  uint32_t NB = nb_all;
+  uint32_t n_src = (uint32_t)std::min<uint64_t>(g->hot_n, (uint64_t)NB * bs);
+  std::vector<uint32_t> n_pref(NB, Nh);
+  uint32_t* d_pref = nullptr;
+  LUXB_TRY(tmp.alloc(&d_pref, kPanelMaxBlocks));
+  LUXB_CUDA(cudaMemcpyAsync(d_pref, n_pref.data(), (size_t)NB * 4, cudaMemcpyHostToDevice, g->stream));
 
-  // cold segments: cold gather ids [H, H + C) cut into S segments of `seg` values, sort keys NB .. NB + S - 1 (<= 254)
+  // cold segments: cold gather ids [H, H + C) cut into S <= 255 - NB0 segments of `seg` values, sort keys NB .. NB + S - 1
   const int cs_mode = g->cold_z ? env_int("LUXB_CS", -1) : 0;
   ColdSplit cs{};
   cs.hot_n = g->hot_n;
@@ -1624,7 +1662,7 @@ static int build_panel_layout(luxb_graph* g) {
   if (cs_mode != 0 && g->cold_n > 0) {
     const char* env = getenv("LUXB_CS_SEG_MB");
     const double seg_mb = env ? atof(env) : 24.0;
-    const uint32_t s_max = 255 - NB;
+    const uint32_t s_max = 255 - NB0;
     uint64_t seg = std::max<uint64_t>(1, (uint64_t)(seg_mb * 1e6 / 4.0));
     seg = std::min<uint64_t>(std::max<uint64_t>(seg, (g->cold_n + s_max - 1) / s_max), g->cold_n);
     S = (uint32_t)((g->cold_n + seg - 1) / seg);
@@ -1633,43 +1671,80 @@ static int build_panel_layout(luxb_graph* g) {
   uint32_t* d_cold_cnt = nullptr;
   if (cs.seg) LUXB_TRY(tmp.alloc(&d_cold_cnt, Nh));
 
-  // 2. edge keys: block of the source for (hot source, hub destination) edges, cold segment + NB for (cold source, hub
-  // destination) edges if the cold split is on, 255 for the rest; 3. stable sort
-  uint8_t *d_key = nullptr, *d_key2 = nullptr;
+  // 2. edge keys: block of the source for (hot source, hub destination in the block's prefix) edges, cold segment + NB
+  // for (cold source, hub destination) edges if the cold split is on, kSplitKeyMain for the rest; 3. stable sort
+  uint16_t *d_key = nullptr, *d_key2 = nullptr;
   uint64_t *d_pay = nullptr, *d_pay2 = nullptr;
   LUXB_TRY(tmp.alloc(&d_key, g->e_part));
   LUXB_TRY(tmp.alloc(&d_key2, g->e_part));
   LUXB_TRY(tmp.alloc(&d_pay, g->e_part));
   LUXB_TRY(tmp.alloc(&d_pay2, g->e_part));
+  constexpr int kBins = kSplitKeyMain + 1;
   unsigned long long* d_hist = nullptr;
-  LUXB_TRY(tmp.alloc(&d_hist, 256));
-  unsigned long long hist[256];
+  LUXB_TRY(tmp.alloc(&d_hist, kBins));
+  unsigned long long hist[kBins];
+  bool tiers_open = tiers && NB > NB0;  // the tier prefixes still have to be chosen from this keying's histogram
   for (;;) {
     edge_iota_kernel<<<grid, 256, 0, g->stream>>>(d_pay, d_key, g->e_part);
-    hub_key_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, g->d_src_gather, d_hub_vtx, Nh, n_src, bs, d_key, d_pay, d_cov, cs, d_cold_cnt);
-    LUXB_CUDA(cudaMemsetAsync(d_hist, 0, 256 * 8, g->stream));
+    hub_key_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, g->d_src_gather, d_hub_vtx, Nh, n_src, bs, d_pref, NB, d_key, d_pay, d_cov,
+                                                cs, d_cold_cnt);
+    LUXB_CUDA(cudaMemsetAsync(d_hist, 0, kBins * 8, g->stream));
     key_hist_kernel<<<grid, 256, 0, g->stream>>>(d_key, g->e_part, d_hist);
     LUXB_CUDA(cudaGetLastError());
     LUXB_CUDA(cudaMemcpyAsync(hist, d_hist, sizeof(hist), cudaMemcpyDeviceToHost, g->stream));
     LUXB_CUDA(cudaStreamSynchronize(g->stream));
+    if (tiers_open) {
+      // block b >= NB0 keeps hub h while d_h * m_b >= slot_edges, m_b = (edges block b -> hubs) / (edges into hubs)
+      tiers_open = false;
+      uint64_t e_hub = 0;
+      for (uint32_t h = 0; h < Nh; ++h) e_hub += ~hub_key[h];
+      for (uint32_t b = NB0; b < NB; ++b) {
+        uint32_t keep = 0;
+        if (hist[b] > 0) {
+          const double d_min = slot_edges * (double)e_hub / (double)hist[b];
+          // hub_key ascends (~in-degree): the hubs with in-degree >= d_min are a prefix
+          keep = (uint32_t)(std::partition_point(hub_key.begin(), hub_key.end(), [&](uint32_t k) { return (double)~k >= d_min; }) - hub_key.begin());
+        }
+        n_pref[b] = std::min(keep, n_pref[b - 1]);
+      }
+      while (NB > NB0 && n_pref[NB - 1] == 0) --NB;
+      n_src = (uint32_t)std::min<uint64_t>(g->hot_n, (uint64_t)NB * bs);
+      cs.key0 = NB;
+      LUXB_CUDA(cudaMemcpyAsync(d_pref, n_pref.data(), (size_t)NB * 4, cudaMemcpyHostToDevice, g->stream));
+      continue;
+    }
     uint64_t e_cs = 0;
     for (uint32_t s = 0; s < S; ++s) e_cs += hist[NB + s];
     if (cs.seg == 0 || cs_mode > 0 || (e_cs > 0 && (double)e_cs >= kColdSplitMinShare * (double)g->e_part)) break;
     cs.seg = 0;  // automatic and too few cold -> hub edges: key again without the cold split
   }
   if (cs.seg == 0) S = 0;
-  tb = 0;
-  LUXB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_key, d_key2, d_pay, d_pay2, (long long)g->e_part, 0, 8, g->stream));
-  LUXB_TRY(tmp.alloc((char**)&d_scan_tmp, tb + 256));
-  LUXB_CUDA(cub::DeviceRadixSort::SortPairs(d_scan_tmp, tb, d_key, d_key2, d_pay, d_pay2, (long long)g->e_part, 0, 8, g->stream));
-  LUXB_CUDA(cudaStreamSynchronize(g->stream));
-  tmp.release(d_scan_tmp);
-  tmp.release(d_key);
-  tmp.release(d_pay);
-  uint64_t e_cov = 0, e_cold = 0;
+  {
+    // two stable sorts: by hub position (payload bits 32.., 0 for main edges), then by key.  Every block and segment
+    // then lists its edges by virtual vertex (hub order is not id order), the main stream keeps the CSC order.
+    cub::DoubleBuffer<uint16_t> kb(d_key, d_key2);
+    cub::DoubleBuffer<uint64_t> pb(d_pay, d_pay2);
+    int hbits = 1;
+    while ((1ull << hbits) < (uint64_t)Nh) ++hbits;
+    size_t tb1 = 0, tb2 = 0;
+    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb1, pb, kb, (long long)g->e_part, 32, 32 + hbits, g->stream));
+    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb2, kb, pb, (long long)g->e_part, 0, kSplitKeyBits, g->stream));
+    tb = std::max(tb1, tb2);
+    LUXB_TRY(tmp.alloc((char**)&d_scan_tmp, tb + 256));
+    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(d_scan_tmp, tb, pb, kb, (long long)g->e_part, 32, 32 + hbits, g->stream));
+    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(d_scan_tmp, tb, kb, pb, (long long)g->e_part, 0, kSplitKeyBits, g->stream));
+    LUXB_CUDA(cudaStreamSynchronize(g->stream));
+    tmp.release(d_scan_tmp);
+    tmp.release(kb.Alternate());
+    tmp.release(pb.Alternate());
+    d_key2 = kb.Current();
+    d_pay2 = pb.Current();
+  }
+  uint64_t e_cov = 0, e_cov0 = 0, e_cold = 0;
   for (uint32_t b = 0; b < NB; ++b) e_cov += hist[b];
+  for (uint32_t b = 0; b < NB0; ++b) e_cov0 += hist[b];
   for (uint32_t s = 0; s < S; ++s) e_cold += hist[NB + s];
-  const uint64_t e_main = hist[255];
+  const uint64_t e_main = hist[kSplitKeyMain];
   if (e_cov + e_cold + e_main != g->e_part) {
     set_error("panel split lost edges (%llu + %llu + %llu != %llu)", (unsigned long long)e_cov, (unsigned long long)e_cold,
               (unsigned long long)e_main, (unsigned long long)g->e_part);
@@ -1677,13 +1752,17 @@ static int build_panel_layout(luxb_graph* g) {
   }
   if (e_cov == 0 || (mode < 0 && e_cov < g->e_part / 5)) return 0;
 
-  // 4. panel CSC over virtual vertices (block b, hub h) -> index b * Nh + h: offsets + per-vertex in-degree
-  const uint32_t NV = Nh * NB;
+  // 4. panel CSC over virtual vertices (block b, hub h < N_b) -> index vbase[b] + h: offsets + per-vertex in-degree
+  uint64_t nv_total = 0;
+  for (uint32_t b = 0; b < NB; ++b) nv_total += n_pref[b];
+  LUXB_ARG(nv_total < 0x7FFFFFF0ull, "panel: too many (block, hub) slots");
+  const uint32_t NV = (uint32_t)nv_total;
   StreamBlocks pblk{};
   pblk.n_blocks = NB;
+  g->sb_pb = PanelBases{};
   for (uint32_t b = 0; b <= NB; ++b) {
-    g->sb_pb.vbase[b] = b * Nh;
-    pblk.vfirst[b] = b * Nh;
+    g->sb_pb.vbase[b] = b == 0 ? 0 : g->sb_pb.vbase[b - 1] + n_pref[b - 1];
+    pblk.vfirst[b] = g->sb_pb.vbase[b];
   }
   pblk.ebase[0] = 0;
   for (uint32_t b = 0; b < NB; ++b) pblk.ebase[b + 1] = pblk.ebase[b] + hist[b];
@@ -1789,14 +1868,18 @@ static int build_panel_layout(luxb_graph* g) {
   g->cs_on = S > 0;
   g->cs_n_seg = S;
   g->cs_seg = cs.seg;
-  g->stats.panel_edges = e_cov;
+  g->stats.panel_edges = e_cov0;
   g->stats.panel_hubs = Nh;
-  g->stats.panel_blocks = NB;
+  g->stats.panel_blocks = NB0;
   g->stats.cold_hub_edges = e_cold;
   g->stats.cold_hub_segments = S;
+  g->stats.tier_blocks = NB - NB0;
+  g->stats.tier_slots = NV - (uint64_t)NB0 * Nh;
+  g->stats.tier_edges = e_cov - e_cov0;
   if (g->cfg.verbose)
-    printf("[luxb rank %d] source-blocked sweep: %u hub destinations (in-degree >= %u) x %u blocks of %u hot sources; panel %llu edges "
-           "(%.1f %%), cold-hub %llu edges (%u segments of %u values), main %llu edges\n", g->cfg.rank, Nh, min_indeg, NB, bs,
+    printf("[luxb rank %d] source-blocked sweep: %u hub destinations (in-degree >= %u) x %u blocks of %u hot sources, + %u tier blocks "
+           "(%llu slots, %llu edges); panel %llu edges (%.1f %%), cold-hub %llu edges (%u segments of %u values), main %llu edges\n",
+           g->cfg.rank, Nh, min_indeg, NB0, bs, NB - NB0, (unsigned long long)(NV - (uint64_t)NB0 * Nh), (unsigned long long)(e_cov - e_cov0),
            (unsigned long long)e_cov, 100.0 * e_cov / g->e_part, (unsigned long long)e_cold, S, cs.seg, (unsigned long long)e_main);
   return 0;
 }

@@ -6,11 +6,14 @@
 // L1 of the lines its misses need.  So the shared-memory gathers get a kernel launch of their own, in which NOTHING
 // goes through L1:
 //
-//   * hub destinations  = local vertices with in-degree >= D (they own most edges of a skewed graph);
+//   * hub destinations  = local vertices with in-degree >= D (they own most edges of a skewed graph), ordered by
+//     in-degree, descending (ties: ascending id);
 //   * hot source blocks = the hot-packed value space [0, Ns) cut into NB blocks of BS <= 32768 values (BS * 4 B fits
 //     shared memory next to the streaming ring);
-//   * every edge (hot source of block b -> hub destination h) moves from the partition's CSC into the PANEL: one
-//     "virtual vertex" b * Nh + h per (block, hub), in that order, its in-edges stored as 15-BIT offsets into block b
+//   * block b serves the hub prefix [0, N_b), N_b not increasing with b ("tiers"): tier 0 = the first blocks over all
+//     hubs; later (less hot) blocks only over the hubs of highest in-degree, where a slot still collects enough edges;
+//   * every edge (hot source of block b -> hub destination h < N_b) moves from the partition's CSC into the PANEL: one
+//     "virtual vertex" vbase[b] + h per (block, hub), in that order, its in-edges stored as 15-BIT offsets into block b
 //     plus a head flag — 2 B of edge stream instead of 4 B.  Blocks are padded to whole stages, so a stage never
 //     straddles two blocks.
 // The panel stream is swept by seg_tile_kernel<kPanel> (seg.cuh): its producer warp keeps block b's values resident in
@@ -25,7 +28,11 @@
 
 namespace luxb {
 
-constexpr int kPanelMaxBlocks = 64;
+// 177 blocks of 32768 values cover a 24 MB hot set; SegArgs / StreamBlocks carry per-block arrays as kernel parameters
+constexpr int kPanelMaxBlocks = 256;
+// 16-bit sort keys of the split: block b -> b, cold segment s -> NB + s (< kSplitKeyMain), main stream -> kSplitKeyMain
+constexpr uint16_t kSplitKeyMain = 511;
+constexpr int kSplitKeyBits = 9;
 
 // ---- one-time construction of the panel / main split --------------------------------------------------------------
 __global__ void hub_flag_kernel(const uint64_t* __restrict__ row_end_rel, uint32_t n_part, uint32_t min_indeg,
@@ -36,8 +43,8 @@ __global__ void hub_flag_kernel(const uint64_t* __restrict__ row_end_rel, uint32
   }
 }
 
-// hub_idx = exclusive scan of flag.  Writes the hub list (local vertex ids, ascending) and the bitmap the main
-// kernel tests (bit v of word v / 32).
+// hub_idx = exclusive scan of flag.  Writes the hub list (local vertex ids, ascending; hub_order_key_kernel and a
+// stable sort then order it by in-degree) and the bitmap the main kernel tests (bit v of word v / 32).
 __global__ void hub_list_kernel(const uint32_t* __restrict__ flag, const uint32_t* __restrict__ hub_idx, uint32_t n_part,
                                 uint32_t* __restrict__ hub_vtx, uint32_t* __restrict__ hub_bits) {
   const uint64_t n_round = ((uint64_t)n_part + 31) & ~31ull;
@@ -49,10 +56,25 @@ __global__ void hub_list_kernel(const uint32_t* __restrict__ flag, const uint32_
   }
 }
 
-__global__ void edge_iota_kernel(uint64_t* __restrict__ payload, uint8_t* __restrict__ key, uint64_t n) {
+// sort key of hub h: its in-degree, descending (a stable ascending sort of ~indeg keeps ascending ids among ties)
+__global__ void hub_order_key_kernel(const uint64_t* __restrict__ row_end_rel, const uint32_t* __restrict__ hub_vtx, uint32_t n_hub,
+                                     uint32_t* __restrict__ key) {
+  for (uint64_t h = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; h < n_hub; h += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t v = hub_vtx[h];
+    key[h] = ~(uint32_t)(row_end_rel[v] - (v == 0 ? 0 : row_end_rel[v - 1]));
+  }
+}
+
+// hub_idx[v] = position of hub v in the ordered hub list (entries of non-hubs are left as they are)
+__global__ void hub_pos_kernel(const uint32_t* __restrict__ hub_vtx, uint32_t n_hub, uint32_t* __restrict__ hub_idx) {
+  for (uint64_t h = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; h < n_hub; h += (uint64_t)gridDim.x * blockDim.x)
+    hub_idx[hub_vtx[h]] = (uint32_t)h;
+}
+
+__global__ void edge_iota_kernel(uint64_t* __restrict__ payload, uint16_t* __restrict__ key, uint64_t n) {
   for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (uint64_t)gridDim.x * blockDim.x) {
     payload[e] = e;
-    key[e] = 255;
+    key[e] = kSplitKeyMain;
   }
 }
 
@@ -68,12 +90,17 @@ struct ColdSplit {
   uint32_t key0;     // sort key of segment 0 (= number of panel blocks)
 };
 
-// one warp per hub vertex: edges whose (hot-packed) source id lies below n_src get key = block, payload = (h, e);
-// with the cold split on, edges whose source is cold get key = cs.key0 + segment
+// one warp per hub h (position in the ordered list): edges whose (hot-packed) source id lies below n_src, in a block b
+// with h < n_pref[b], get key = b, payload = (h, e); with the cold split on, edges whose source is cold get key =
+// cs.key0 + segment.  n_pref: [n_blocks] hub prefix of each block, n_blocks <= kPanelMaxBlocks.
 __global__ void hub_key_kernel(const uint64_t* __restrict__ row_end_rel, const uint32_t* __restrict__ src_gather,
                                const uint32_t* __restrict__ hub_vtx, uint32_t n_hub, uint32_t n_src, uint32_t bs,
-                               uint8_t* __restrict__ key, uint64_t* __restrict__ payload, uint32_t* __restrict__ cov_count,
+                               const uint32_t* __restrict__ n_pref, uint32_t n_blocks,
+                               uint16_t* __restrict__ key, uint64_t* __restrict__ payload, uint32_t* __restrict__ cov_count,
                                const ColdSplit cs, uint32_t* __restrict__ cold_count) {
+  __shared__ uint32_t s_pref[kPanelMaxBlocks];
+  for (uint32_t i = threadIdx.x; i < n_blocks; i += blockDim.x) s_pref[i] = n_pref[i];
+  __syncthreads();
   const unsigned lane = threadIdx.x & 31;
   const uint64_t warps_total = ((uint64_t)gridDim.x * blockDim.x) >> 5;
   for (uint64_t h = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; h < n_hub; h += warps_total) {
@@ -83,11 +110,13 @@ __global__ void hub_key_kernel(const uint64_t* __restrict__ row_end_rel, const u
     for (uint64_t k = b + lane; k < e; k += 32) {
       const uint32_t id = src_gather[k];
       if (id < n_src) {
-        key[k] = (uint8_t)(id / bs);
-        payload[k] = (h << 32) | k;
-        ++cnt;
+        if (h < s_pref[id / bs]) {
+          key[k] = (uint16_t)(id / bs);
+          payload[k] = (h << 32) | k;
+          ++cnt;
+        }
       } else if (cs.seg != 0 && id >= cs.hot_n) {
-        key[k] = (uint8_t)(cs.key0 + (id - cs.hot_n) / cs.seg);
+        key[k] = (uint16_t)(cs.key0 + (id - cs.hot_n) / cs.seg);
         payload[k] = (h << 32) | k;
         ++ccnt;
       }
@@ -104,24 +133,25 @@ __global__ void hub_key_kernel(const uint64_t* __restrict__ row_end_rel, const u
   }
 }
 
-__global__ void key_hist_kernel(const uint8_t* __restrict__ key, uint64_t n, unsigned long long* __restrict__ hist) {
-  __shared__ unsigned int s_h[256];
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) s_h[i] = 0;
+__global__ void key_hist_kernel(const uint16_t* __restrict__ key, uint64_t n, unsigned long long* __restrict__ hist) {
+  constexpr int kBins = kSplitKeyMain + 1;
+  __shared__ unsigned int s_h[kBins];
+  for (int i = threadIdx.x; i < kBins; i += blockDim.x) s_h[i] = 0;
   __syncthreads();
   // per-CTA counts stay below 2^32: each CTA sees at most n / gridDim.x + blockDim.x keys (n < 2^32 * gridDim.x)
   for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (uint64_t)gridDim.x * blockDim.x)
     atomicAdd(&s_h[key[e]], 1u);
   __syncthreads();
-  for (int i = threadIdx.x; i < 256; i += blockDim.x)
+  for (int i = threadIdx.x; i < kBins; i += blockDim.x)
     if (s_h[i]) atomicAdd(hist + i, (unsigned long long)s_h[i]);
 }
 
 struct PanelBases {
-  uint32_t vbase[kPanelMaxBlocks + 1];  // first virtual vertex of block b; [n_blocks] = NV
+  uint32_t vbase[kPanelMaxBlocks + 1];  // first virtual vertex of block b (its hub prefix: vbase[b + 1] - vbase[b]); [n_blocks] = NV
 };
 
 // sorted (by block, stable) covered edges -> 16-bit offsets + per-virtual-vertex in-degree
-__global__ void panel_fill_kernel(const uint8_t* __restrict__ key_sorted, const uint64_t* __restrict__ payload_sorted,
+__global__ void panel_fill_kernel(const uint16_t* __restrict__ key_sorted, const uint64_t* __restrict__ payload_sorted,
                                   uint64_t e_cov, const uint32_t* __restrict__ src_gather, uint32_t bs,
                                   const __grid_constant__ PanelBases pb, uint16_t* __restrict__ src16, uint32_t* __restrict__ vcount) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < e_cov; i += (uint64_t)gridDim.x * blockDim.x) {
@@ -134,7 +164,7 @@ __global__ void panel_fill_kernel(const uint8_t* __restrict__ key_sorted, const 
 }
 
 // sorted (by segment, stable) cold-hub edges -> their gather ids unchanged + per-virtual-vertex (s * Nh + h) in-degree
-__global__ void cold_fill_kernel(const uint8_t* __restrict__ key_sorted, const uint64_t* __restrict__ payload_sorted, uint64_t e_cold,
+__global__ void cold_fill_kernel(const uint16_t* __restrict__ key_sorted, const uint64_t* __restrict__ payload_sorted, uint64_t e_cold,
                                  const uint32_t* __restrict__ src_gather, uint32_t key0, uint32_t n_hub, uint32_t* __restrict__ ids,
                                  uint32_t* __restrict__ vcount) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < e_cold; i += (uint64_t)gridDim.x * blockDim.x) {
@@ -163,7 +193,8 @@ __global__ void main_indeg_kernel(const uint64_t* __restrict__ row_end_rel, uint
   }
 }
 
-// ---- per-iteration: hubs = main raw sum + panel partials + cold-segment partials, fp64, fixed order; then update() ---
+// ---- per-iteration: hubs = main raw sum + panel partials (blocks b with h < N_b) + cold-segment partials, fp64, fixed
+// order; then update() ---
 template <class Prog>
 struct CombineArgs {
   const uint32_t* hub_vtx;   // [n_hub] local vertex ids
@@ -184,7 +215,19 @@ __global__ void combine_hub_kernel(const __grid_constant__ CombineArgs<Prog> a) 
     typename Prog::Acc raw0;
     memcpy(&raw0, &a.out[v], sizeof(raw0));  // the main sweep left its RAW reduction in the value slot
     typename Prog::Wide t = Prog::widen(raw0);
-    for (uint32_t b = 0; b < a.n_blocks; ++b) t = Prog::wcombine(t, Prog::widen(a.partial[a.pb.vbase[b] + h]));
+    // block b has a slot for h while h < N_b; N_b does not increase with b, so h < N_{b+7} means blocks b .. b+7 all
+    // have one: their loads are issued together, the adds keep block order.  Hubs are ordered by in-degree, so the
+    // threads of a warp run about the same number of blocks.
+    uint32_t b = 0;
+    for (; b + 8 <= a.n_blocks && h < a.pb.vbase[b + 8] - a.pb.vbase[b + 7]; b += 8) {
+      typename Prog::Acc p[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) p[i] = a.partial[a.pb.vbase[b + i] + h];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) t = Prog::wcombine(t, Prog::widen(p[i]));
+    }
+    for (; b < a.n_blocks && h < a.pb.vbase[b + 1] - a.pb.vbase[b]; ++b)
+      t = Prog::wcombine(t, Prog::widen(a.partial[a.pb.vbase[b] + h]));
     for (uint32_t s = 0; s < a.n_cold_seg; ++s) t = Prog::wcombine(t, Prog::widen(a.cold_partial[(uint64_t)s * a.n_hub + h]));
     const typename Prog::Vertex oldv = Prog::kNeedsOld ? a.x_nat[a.row_left + v] : typename Prog::Vertex();
     const typename Prog::Vertex nv_ = Prog::update(a.row_left + v, Prog::narrow(t), oldv, a.prm);

@@ -329,6 +329,17 @@ struct StreamBlocks {            // vertices [vfirst[b], vfirst[b+1]) live in bl
   uint64_t hshift[kPanelMaxBlocks + 1];  // pad heads inserted before block b
 };
 
+// the last block b < n with first[b] <= x (first[0] <= x; blocks may be empty)
+template <class T>
+__device__ __forceinline__ uint32_t find_block(const T* first, uint32_t n, uint64_t x) {
+  uint32_t lo = 0, hi = n;  // first[lo] <= x, and first[hi] > x or hi == n
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if ((uint64_t)first[mid] <= x) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
 __global__ void nonempty_flag_kernel(const uint64_t* __restrict__ row_end, uint32_t n_vtx, uint32_t* __restrict__ flag) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_vtx; i += (uint64_t)gridDim.x * blockDim.x)
     flag[i] = row_end[i] > (i == 0 ? 0 : row_end[i - 1]) ? 1u : 0u;
@@ -341,8 +352,7 @@ __global__ void stream_heads_kernel(const uint64_t* __restrict__ row_end, uint32
   constexpr Word kHead = (Word)1 << (sizeof(Word) * 8 - 1);
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_vtx; i += (uint64_t)gridDim.x * blockDim.x) {
     if (!flag[i]) continue;
-    uint32_t b = 0;
-    while (b + 1 < sb.n_blocks && i >= sb.vfirst[b + 1]) ++b;
+    const uint32_t b = find_block(sb.vfirst, sb.n_blocks, i);
     const uint64_t begin = i == 0 ? 0 : row_end[i - 1];
     words[begin - sb.ebase[b] + sb.wbase[b]] |= kHead;
     close_list[1 + (uint64_t)segrank[i] + sb.hshift[b]] = (uint32_t)i + vtx_offset;
@@ -354,8 +364,7 @@ template <class Word, class In>
 __global__ void stream_copy_kernel(const In* __restrict__ ids, uint64_t e_cnt, const __grid_constant__ StreamBlocks sb,
                                    Word* __restrict__ words) {
   for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < e_cnt; e += (uint64_t)gridDim.x * blockDim.x) {
-    uint32_t b = 0;
-    while (b + 1 < sb.n_blocks && e >= sb.ebase[b + 1]) ++b;
+    const uint32_t b = find_block(sb.ebase, sb.n_blocks, e);
     words[e - sb.ebase[b] + sb.wbase[b]] = (Word)ids[e];
   }
 }

@@ -63,6 +63,7 @@ for c in cfgs:
         err = (np.abs(x6[blk["vid"]].astype(np.float64) - ref) / np.abs(ref.astype(np.float64))).max()
         k = (s1["dominant_kernel_seconds"] - s0["dominant_kernel_seconds"]) / 20
         t = (s1["loop_seconds"] - s0["loop_seconds"]) / 20
-        print("cfg %-40s panel %.1f%% of edges, %d hubs x %d blocks | sweep %.3f ms, iter %.3f ms, %.1f GTEPS, frac %.3f | parity %.2e %s" % (
-            c_label, 100.0 * st["panel_edges"] / ne, st["panel_hubs"], st["panel_blocks"], k * 1e3, t * 1e3, ne / t / 1e9,
+        print("cfg %-40s panel %.1f%% of edges, %d hubs x %d blocks, tiers %d blocks %d slots %.1f%% of edges | sweep %.3f ms, iter %.3f ms, %.1f GTEPS, frac %.3f | parity %.2e %s" % (
+            c_label, 100.0 * st["panel_edges"] / ne, st["panel_hubs"], st["panel_blocks"], st["tier_blocks"], st["tier_slots"],
+            100.0 * st["tier_edges"] / ne, k * 1e3, t * 1e3, ne / t / 1e9,
             (8 * ne + 16 * nv) / k / 1e9 / 6486.8, err, "OK" if err <= 1e-6 else "FAIL"), flush=True)
