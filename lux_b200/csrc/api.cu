@@ -125,6 +125,58 @@ static int edge_alloc(luxb_graph* g, T** p, uint64_t count) {
   return 0;
 }
 
+// temporaries of a build step: freed on every exit path
+struct DevTmp {
+  std::vector<void*> ptrs;
+  ~DevTmp() { for (void* q : ptrs) cudaFree(q); }
+  template <class T>
+  int alloc(T** out, uint64_t count) {
+    LUXB_TRY(dmalloc(out, count));
+    ptrs.push_back(*out);
+    return 0;
+  }
+  void release(void* q) {
+    for (size_t i = 0; i < ptrs.size(); ++i)
+      if (ptrs[i] == q) { cudaFree(q); ptrs.erase(ptrs.begin() + i); return; }
+  }
+  void keep(void* q) {  // ownership moves to the graph
+    for (size_t i = 0; i < ptrs.size(); ++i)
+      if (ptrs[i] == q) { ptrs.erase(ptrs.begin() + i); return; }
+  }
+};
+
+// one two-phase cub call f(temp, bytes) on `stream`: size query, temporary storage from `tmp`, the call; the storage is
+// released once the stream has finished with it
+template <class F>
+static int cub_call(DevTmp& tmp, cudaStream_t stream, F&& f) {
+  size_t bytes = 0;
+  LUXB_CUDA(f(nullptr, bytes));
+  char* d_tmp = nullptr;
+  LUXB_TRY(tmp.alloc(&d_tmp, bytes));
+  LUXB_CUDA(f(d_tmp, bytes));
+  LUXB_CUDA(cudaStreamSynchronize(stream));
+  tmp.release(d_tmp);
+  return 0;
+}
+
+// fix-up scratch of a sweep over n_tiles tiles; the fused fix-up adds its chain on first use (launch_fixup)
+static int alloc_fixup(FixupScratch& f, uint32_t n_tiles) {
+  LUXB_TRY(dmalloc((uint32_t**)&f.d_head, (uint64_t)n_tiles + 1));
+  LUXB_TRY(dmalloc((uint32_t**)&f.d_tail, (uint64_t)n_tiles + 1));
+  f.n_fix_blocks = (n_tiles + kFixBlock - 1) / kFixBlock;
+  LUXB_TRY(dmalloc((uint64_t**)&f.d_carry, (uint64_t)n_tiles + 1));
+  LUXB_TRY(dmalloc(&f.d_carry_flag, (uint64_t)n_tiles + 1));
+  LUXB_TRY(dmalloc((uint64_t**)&f.d_block_agg, (uint64_t)f.n_fix_blocks + 1));
+  LUXB_TRY(dmalloc(&f.d_block_flag, (uint64_t)f.n_fix_blocks + 1));
+  return 0;
+}
+
+static void free_fixup(FixupScratch& f) {
+  for (void* q : {f.d_head, f.d_tail, f.d_carry, (void*)f.d_carry_flag, f.d_block_agg, (void*)f.d_block_flag, (void*)f.d_chain})
+    if (q) cudaFree(q);
+  f = FixupScratch();
+}
+
 // ---- the reference partitioner on the host (pull_model.inl:108-131); same cut rule as partition_kernel -------
 static int host_partition(uint32_t nv, uint64_t ne, const uint64_t* row_end, int P, uint32_t* rl, uint32_t* np,
                           uint64_t* cl) {
@@ -195,7 +247,7 @@ static bool is_label_app(luxb_app app) { return app == LUXB_CC || app == LUXB_SS
 // apps that read the CSC's edge weights
 static bool uses_weights(luxb_app app) { return app == LUXB_COLFILTER || app == LUXB_SSSP_WEIGHTED; }
 
-static int graph_begin(const luxb_config* cfg, luxb_graph** out) {
+static int graph_begin(const luxb_config* cfg, uint32_t nv, uint64_t ne, luxb_graph** out) {
   LUXB_TRY(check_config(cfg));
   LUXB_ARG(out != nullptr, "out is NULL");
   int ndev = 0;
@@ -210,6 +262,9 @@ static int graph_begin(const luxb_config* cfg, luxb_graph** out) {
   if (!g) { set_error("out of host memory"); return LUXB_ERR_NOMEM; }
   g->cfg = *cfg;
   g->P = cfg->nranks;
+  g->nv = nv;
+  g->ne = ne;
+  g->weighted = uses_weights(cfg->app);
   *out = g;
   LUXB_CUDA(cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
   LUXB_CUDA(cudaEventCreate(&g->ev_begin));
@@ -247,6 +302,23 @@ static void set_partition_derived(luxb_graph* g) {
   g->fq_total = off;
 }
 
+// the work split is the reference's split (no cfg.balanced_split)
+static void use_reference_split(luxb_graph* g) {
+  for (int p = 0; p < g->P; ++p) { g->rl[p] = g->ref_rl[p]; g->np[p] = g->ref_np[p]; g->cl[p] = g->ref_cl[p]; }
+}
+
+// open of a CSC whose row_end is in host memory: the graph, both splits and this rank's share of them.  On failure the
+// caller closes *out if it is set.
+static int open_host_begin(const luxb_config* cfg, uint32_t nv, uint64_t ne, const uint64_t* row_end, luxb_graph** out) {
+  LUXB_TRY(graph_begin(cfg, nv, ne, out));
+  luxb_graph* g = *out;
+  g->parts_found = host_partition(nv, ne, row_end, g->P, g->ref_rl, g->ref_np, g->ref_cl);
+  if (use_balanced_split(cfg)) host_balanced_partition(nv, ne, row_end, g->P, g->rl, g->np, g->cl);
+  else use_reference_split(g);
+  set_partition_derived(g);
+  return 0;
+}
+
 // after d_row_end / d_src are in place: merge-path tile table + per-tile partial buffers
 static int finish_layout(luxb_graph* g) {
   uint64_t total = (uint64_t)g->n_part + g->e_part;
@@ -258,22 +330,20 @@ static int finish_layout(luxb_graph* g) {
   const uint32_t tile = (uint32_t)kPullTileOf[g->pull_shape];
   uint64_t nt = (total + tile - 1) / tile;
   LUXB_ARG(nt < 0xFFFFFFFFull, "partition too large for the tile table");
-  g->n_tiles = (uint32_t)nt;
-  LUXB_TRY(dmalloc(&g->d_tile_v, (uint64_t)g->n_tiles + 2));
-  tile_table_kernel<<<grid_for((uint64_t)g->n_tiles + 1, 256, 1 << 20), 256, 0, g->stream>>>(
-      g->d_row_end, g->n_part, g->e_part, tile, g->n_tiles, g->d_tile_v);
+  PullLayout& B = g->base;
+  B.d_row_end = g->d_row_end;
+  B.n_vtx = g->n_part;
+  B.e_cnt = g->e_part;
+  B.n_tiles = (uint32_t)nt;
+  LUXB_TRY(dmalloc(&B.d_tile_v, (uint64_t)B.n_tiles + 2));
+  tile_table_kernel<<<grid_for((uint64_t)B.n_tiles + 1, 256, 1 << 20), 256, 0, g->stream>>>(
+      g->d_row_end, g->n_part, g->e_part, tile, B.n_tiles, B.d_tile_v);
   LUXB_CUDA(cudaGetLastError());
-  LUXB_TRY(dmalloc(&g->d_row_end32, (uint64_t)g->n_part + 8));
+  LUXB_TRY(dmalloc(&B.d_row_end32, (uint64_t)g->n_part + 8));
   narrow_u64_to_u32_kernel<<<grid_for((uint64_t)g->n_part + 8, 256, 4096), 256, 0, g->stream>>>(g->d_row_end, g->n_part + 4,
-                                                                                          g->d_row_end32, (uint64_t)g->n_part + 8);
+                                                                                          B.d_row_end32, (uint64_t)g->n_part + 8);
   LUXB_CUDA(cudaGetLastError());
-  LUXB_TRY(dmalloc((uint32_t**)&g->d_head, (uint64_t)g->n_tiles + 1));
-  LUXB_TRY(dmalloc((uint32_t**)&g->d_tail, (uint64_t)g->n_tiles + 1));
-  g->n_fix_blocks = (g->n_tiles + kFixBlock - 1) / kFixBlock;
-  LUXB_TRY(dmalloc((uint64_t**)&g->d_carry, (uint64_t)g->n_tiles + 1));
-  LUXB_TRY(dmalloc(&g->d_carry_flag, (uint64_t)g->n_tiles + 1));
-  LUXB_TRY(dmalloc((uint64_t**)&g->d_block_agg, (uint64_t)g->n_fix_blocks + 1));
-  LUXB_TRY(dmalloc(&g->d_block_flag, (uint64_t)g->n_fix_blocks + 1));
+  LUXB_TRY(alloc_fixup(B.fix, B.n_tiles));
   LUXB_TRY(dmalloc(&g->d_counters, 8));  // [0] edges scanned, [1] check mistakes, [2] pull tile counter, [3] big segments, [4] panel / cold-hub tile counter
   LUXB_CUDA(cudaMemsetAsync(g->d_counters, 0, 8 * sizeof(unsigned long long), g->stream));
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
@@ -355,15 +425,8 @@ int luxb_open_csc(const luxb_csc* csc, const luxb_config* cfg, luxb_graph** out)
   LUXB_ARG(cfg->app != LUXB_SSSP_WEIGHTED || csc->weight || csc->ne == 0, "weighted SSSP needs edge weights");
   LUXB_TRY(validate_row_end(csc->nv, csc->ne, csc->row_end));
   luxb_graph* g = nullptr;
-  int rc = graph_begin(cfg, &g);
+  int rc = open_host_begin(cfg, csc->nv, csc->ne, csc->row_end, &g);
   if (rc) { if (g) luxb_close(g); return rc; }
-  g->nv = csc->nv;
-  g->ne = csc->ne;
-  g->weighted = uses_weights(cfg->app);
-  g->parts_found = host_partition(g->nv, g->ne, csc->row_end, g->P, g->ref_rl, g->ref_np, g->ref_cl);
-  if (use_balanced_split(cfg)) host_balanced_partition(g->nv, g->ne, csc->row_end, g->P, g->rl, g->np, g->cl);
-  else for (int p = 0; p < g->P; ++p) { g->rl[p] = g->ref_rl[p]; g->np[p] = g->ref_np[p]; g->cl[p] = g->ref_cl[p]; }
-  set_partition_derived(g);
   rc = upload_slice(g, csc->row_end + (g->n_part ? g->row_left : 0), csc->src + g->col_left,
                     g->weighted ? csc->weight + g->col_left : nullptr);
   if (rc) { luxb_close(g); return rc; }
@@ -388,15 +451,8 @@ int luxb_open_file(const char* path, const luxb_config* cfg, luxb_graph** out) {
   int rc = validate_row_end(nv, ne, row_end.data());
   if (rc) { fclose(f); return rc; }
   luxb_graph* g = nullptr;
-  rc = graph_begin(cfg, &g);
+  rc = open_host_begin(cfg, nv, ne, row_end.data(), &g);
   if (rc) { fclose(f); if (g) luxb_close(g); return rc; }
-  g->nv = nv;
-  g->ne = ne;
-  g->weighted = uses_weights(cfg->app);
-  g->parts_found = host_partition(nv, ne, row_end.data(), g->P, g->ref_rl, g->ref_np, g->ref_cl);
-  if (use_balanced_split(cfg)) host_balanced_partition(nv, ne, row_end.data(), g->P, g->rl, g->np, g->cl);
-  else for (int p = 0; p < g->P; ++p) { g->rl[p] = g->ref_rl[p]; g->np[p] = g->ref_np[p]; g->cl[p] = g->ref_cl[p]; }
-  set_partition_derived(g);
   // this rank's slice only — same seeks as pull_load_task_impl (pull_model.inl:294-318)
   std::vector<uint32_t> src(g->e_part ? g->e_part : 1);
   std::vector<int32_t> w(g->weighted && g->e_part ? g->e_part : 1);
@@ -471,121 +527,103 @@ int luxb_convert_edgelist(const char* edge_list_path, const char* lux_path, luxb
   return luxb_write_lux(lux_path, &csc);
 }
 
-static int open_generated(const GenSpec& spec, const luxb_config* cfg, luxb_graph** out) {
-  luxb_graph* g = nullptr;
-  int rc = graph_begin(cfg, &g);
-  if (rc) { if (g) luxb_close(g); return rc; }
-  auto fail = [&](int code) { luxb_close(g); return code; };
-  g->nv = spec.nv;
-  g->ne = spec.ne;
-  g->weighted = uses_weights(cfg->app);
+// a generated graph (GenSpec): partition table and this rank's slice, built on the device
+static int generate_slice(luxb_graph* g, const GenSpec& spec) {
+  DevTmp tmp;
   const int gen_grid = g->num_sms * 16;
   // 1. in-degree histogram over the whole edge stream -> global row_end (u64) by an inclusive scan
   uint32_t* d_indeg = nullptr;
   uint64_t* d_row_end_g = nullptr;
-  if ((rc = dmalloc(&d_indeg, spec.nv))) return fail(rc);
-  if ((rc = dmalloc(&d_row_end_g, spec.nv))) return fail(rc);
-#define GEN_CUDA(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { set_error("CUDA error %s: %s", #x, cudaGetErrorString(_e)); return fail(LUXB_ERR_CUDA); } } while (0)
-  GEN_CUDA(cudaMemsetAsync(d_indeg, 0, (size_t)spec.nv * 4, g->stream));
+  LUXB_TRY(tmp.alloc(&d_indeg, spec.nv));
+  LUXB_TRY(tmp.alloc(&d_row_end_g, spec.nv));
+  LUXB_CUDA(cudaMemsetAsync(d_indeg, 0, (size_t)spec.nv * 4, g->stream));
   gen_count_indeg_kernel<<<gen_grid, 256, 0, g->stream>>>(spec, d_indeg);
   widen_u32_to_u64_kernel<<<gen_grid, 256, 0, g->stream>>>(d_indeg, d_row_end_g, spec.nv);
-  size_t tmp_bytes = 0;
-  GEN_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, d_row_end_g, d_row_end_g, (int)spec.nv, g->stream));
-  void* d_tmp = nullptr;
-  GEN_CUDA(cudaMalloc(&d_tmp, tmp_bytes + 256));
-  GEN_CUDA(cub::DeviceScan::InclusiveSum(d_tmp, tmp_bytes, d_row_end_g, d_row_end_g, (int)spec.nv, g->stream));
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceScan::InclusiveSum(t, b, d_row_end_g, d_row_end_g, (int)spec.nv, g->stream);
+  }));
   // 2. partition table (reference greedy split), on the device
   uint32_t* d_pt = nullptr;  // rl[P], np[P]
   uint64_t* d_cl = nullptr;
   int* d_cnt = nullptr;
-  if ((rc = dmalloc(&d_pt, 2 * LUXB_MAX_PARTS))) return fail(rc);
-  if ((rc = dmalloc(&d_cl, LUXB_MAX_PARTS))) return fail(rc);
-  if ((rc = dmalloc(&d_cnt, 1))) return fail(rc);
+  LUXB_TRY(tmp.alloc(&d_pt, 2 * LUXB_MAX_PARTS));
+  LUXB_TRY(tmp.alloc(&d_cl, LUXB_MAX_PARTS));
+  LUXB_TRY(tmp.alloc(&d_cnt, 1));
   partition_kernel<<<1, 1, 0, g->stream>>>(d_row_end_g, spec.nv, spec.ne, g->P, d_pt, d_pt + LUXB_MAX_PARTS, d_cl, d_cnt);
-  GEN_CUDA(cudaMemcpyAsync(g->ref_rl, d_pt, g->P * 4, cudaMemcpyDeviceToHost, g->stream));
-  GEN_CUDA(cudaMemcpyAsync(g->ref_np, d_pt + LUXB_MAX_PARTS, g->P * 4, cudaMemcpyDeviceToHost, g->stream));
-  GEN_CUDA(cudaMemcpyAsync(g->ref_cl, d_cl, g->P * 8, cudaMemcpyDeviceToHost, g->stream));
-  GEN_CUDA(cudaMemcpyAsync(&g->parts_found, d_cnt, 4, cudaMemcpyDeviceToHost, g->stream));
-  GEN_CUDA(cudaStreamSynchronize(g->stream));
-  if (use_balanced_split(cfg)) {
+  LUXB_CUDA(cudaMemcpyAsync(g->ref_rl, d_pt, g->P * 4, cudaMemcpyDeviceToHost, g->stream));
+  LUXB_CUDA(cudaMemcpyAsync(g->ref_np, d_pt + LUXB_MAX_PARTS, g->P * 4, cudaMemcpyDeviceToHost, g->stream));
+  LUXB_CUDA(cudaMemcpyAsync(g->ref_cl, d_cl, g->P * 8, cudaMemcpyDeviceToHost, g->stream));
+  LUXB_CUDA(cudaMemcpyAsync(&g->parts_found, d_cnt, 4, cudaMemcpyDeviceToHost, g->stream));
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  if (use_balanced_split(&g->cfg)) {
     // cost prefix over all vertices (in place of the in-degree scratch), then P - 1 binary searches for the cut points
     uint64_t* d_cost = nullptr;
-    if ((rc = dmalloc(&d_cost, (uint64_t)spec.nv + 1))) return fail(rc);
+    LUXB_TRY(tmp.alloc(&d_cost, (uint64_t)spec.nv + 1));
     vertex_cost_kernel<<<gen_grid, 256, 0, g->stream>>>(d_row_end_g, spec.nv, kBalanceHubIndeg, d_cost);
-    size_t tb2 = 0;
-    GEN_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb2, d_cost, d_cost, (int)spec.nv, g->stream));
-    void* d_tmp2 = nullptr;
-    GEN_CUDA(cudaMalloc(&d_tmp2, tb2 + 256));
-    GEN_CUDA(cub::DeviceScan::InclusiveSum(d_tmp2, tb2, d_cost, d_cost, (int)spec.nv, g->stream));
+    LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+      return cub::DeviceScan::InclusiveSum(t, b, d_cost, d_cost, (int)spec.nv, g->stream);
+    }));
     balanced_cut_kernel<<<1, 1, 0, g->stream>>>(d_cost, d_row_end_g, spec.nv, spec.ne, g->P, d_pt, d_pt + LUXB_MAX_PARTS, d_cl);
-    GEN_CUDA(cudaMemcpyAsync(g->rl, d_pt, g->P * 4, cudaMemcpyDeviceToHost, g->stream));
-    GEN_CUDA(cudaMemcpyAsync(g->np, d_pt + LUXB_MAX_PARTS, g->P * 4, cudaMemcpyDeviceToHost, g->stream));
-    GEN_CUDA(cudaMemcpyAsync(g->cl, d_cl, g->P * 8, cudaMemcpyDeviceToHost, g->stream));
-    GEN_CUDA(cudaStreamSynchronize(g->stream));
-    GEN_CUDA(cudaFree(d_tmp2));
-    GEN_CUDA(cudaFree(d_cost));
+    LUXB_CUDA(cudaMemcpyAsync(g->rl, d_pt, g->P * 4, cudaMemcpyDeviceToHost, g->stream));
+    LUXB_CUDA(cudaMemcpyAsync(g->np, d_pt + LUXB_MAX_PARTS, g->P * 4, cudaMemcpyDeviceToHost, g->stream));
+    LUXB_CUDA(cudaMemcpyAsync(g->cl, d_cl, g->P * 8, cudaMemcpyDeviceToHost, g->stream));
+    LUXB_CUDA(cudaStreamSynchronize(g->stream));
+    tmp.release(d_cost);
   } else {
-    for (int p = 0; p < g->P; ++p) { g->rl[p] = g->ref_rl[p]; g->np[p] = g->ref_np[p]; g->cl[p] = g->ref_cl[p]; }
+    use_reference_split(g);
   }
   set_partition_derived(g);
   // 3. local row_end (relative + sentinels)
-  if ((rc = dmalloc(&g->d_row_end, (uint64_t)g->n_part + 4))) return fail(rc);
+  LUXB_TRY(dmalloc(&g->d_row_end, (uint64_t)g->n_part + 4));
   rowend_rel_kernel<<<grid_for((uint64_t)g->n_part + 4, 256, 4096), 256, 0, g->stream>>>(d_row_end_g, g->row_left, g->n_part,
                                                                                         g->col_left, g->d_row_end);
-  GEN_CUDA(cudaGetLastError());
-  GEN_CUDA(cudaStreamSynchronize(g->stream));
-  GEN_CUDA(cudaFree(d_indeg));
-  GEN_CUDA(cudaFree(d_row_end_g));
-  GEN_CUDA(cudaFree(d_tmp));
-  GEN_CUDA(cudaFree(d_pt));
-  GEN_CUDA(cudaFree(d_cl));
-  GEN_CUDA(cudaFree(d_cnt));
+  LUXB_CUDA(cudaGetLastError());
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  for (void* q : {(void*)d_indeg, (void*)d_row_end_g, (void*)d_pt, (void*)d_cl, (void*)d_cnt}) tmp.release(q);
   // 4. this partition's edges: regenerate the stream, keep keys (dst_local << 32 | src), radix sort -> canonical CSC
   uint64_t *d_keys = nullptr, *d_keys_alt = nullptr;
   unsigned long long* d_cursor = nullptr;
-  if ((rc = dmalloc(&d_keys, g->e_part))) return fail(rc);
-  if ((rc = dmalloc(&d_keys_alt, g->e_part))) return fail(rc);
-  if ((rc = dmalloc(&d_cursor, 1))) return fail(rc);
-  GEN_CUDA(cudaMemsetAsync(d_cursor, 0, 8, g->stream));
+  LUXB_TRY(tmp.alloc(&d_keys, g->e_part));
+  LUXB_TRY(tmp.alloc(&d_keys_alt, g->e_part));
+  LUXB_TRY(tmp.alloc(&d_cursor, 1));
+  LUXB_CUDA(cudaMemsetAsync(d_cursor, 0, 8, g->stream));
   gen_emit_keys_kernel<<<gen_grid, 256, 0, g->stream>>>(spec, g->row_left, g->n_part, d_cursor, d_keys, g->e_part);
-  GEN_CUDA(cudaGetLastError());
+  LUXB_CUDA(cudaGetLastError());
   unsigned long long emitted = 0;
-  GEN_CUDA(cudaMemcpyAsync(&emitted, d_cursor, 8, cudaMemcpyDeviceToHost, g->stream));
-  GEN_CUDA(cudaStreamSynchronize(g->stream));
+  LUXB_CUDA(cudaMemcpyAsync(&emitted, d_cursor, 8, cudaMemcpyDeviceToHost, g->stream));
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
   if (emitted != g->e_part) {
     set_error("generator emitted %llu edges for this partition, expected %llu", emitted, (unsigned long long)g->e_part);
-    return fail(LUXB_ERR_STATE);
+    return LUXB_ERR_STATE;
   }
-  int vbits = 1;
-  while ((1ull << vbits) < (uint64_t)spec.nv) ++vbits;
   int pbits = 1;
   while ((1ull << pbits) < (uint64_t)g->n_part + 1) ++pbits;
   cub::DoubleBuffer<uint64_t> keys(d_keys, d_keys_alt);
-  tmp_bytes = 0;
-  GEN_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, keys, (long long)g->e_part, 0, 32 + pbits, g->stream));
-  GEN_CUDA(cudaMalloc(&d_tmp, tmp_bytes + 256));
-  GEN_CUDA(cub::DeviceRadixSort::SortKeys(d_tmp, tmp_bytes, keys, (long long)g->e_part, 0, 32 + pbits, g->stream));
-  if ((rc = edge_alloc(g, &g->d_src, g->e_part + 8))) return fail(rc);
-  GEN_CUDA(cudaMemsetAsync(g->d_src, 0, (g->e_part + 8) * 4, g->stream));
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortKeys(t, b, keys, (long long)g->e_part, 0, 32 + pbits, g->stream);
+  }));
+  LUXB_TRY(edge_alloc(g, &g->d_src, g->e_part + 8));
+  LUXB_CUDA(cudaMemsetAsync(g->d_src, 0, (g->e_part + 8) * 4, g->stream));
   if (g->weighted) {
-    if ((rc = edge_alloc(g, &g->d_weight, g->e_part + 8))) return fail(rc);
-    GEN_CUDA(cudaMemsetAsync(g->d_weight, 0, (g->e_part + 8) * 4, g->stream));
+    LUXB_TRY(edge_alloc(g, &g->d_weight, g->e_part + 8));
+    LUXB_CUDA(cudaMemsetAsync(g->d_weight, 0, (g->e_part + 8) * 4, g->stream));
   }
   // bipartite: the ratings 1..5 of the (user, item) pair; RMAT (weighted SSSP): directed weights 1..255
   keys_to_src_kernel<<<gen_grid, 256, 0, g->stream>>>(keys.Current(), g->e_part, g->d_src, spec.kind == 0 ? nullptr : g->d_weight,
                                                       spec.seed, g->row_left);
   if (spec.kind == 0 && g->weighted)
     keys_to_rmat_weight_kernel<<<gen_grid, 256, 0, g->stream>>>(keys.Current(), g->e_part, g->d_weight, spec.seed, g->row_left);
-  GEN_CUDA(cudaGetLastError());
-  GEN_CUDA(cudaStreamSynchronize(g->stream));
-  GEN_CUDA(cudaFree(d_keys));
-  GEN_CUDA(cudaFree(d_keys_alt));
-  GEN_CUDA(cudaFree(d_cursor));
-  GEN_CUDA(cudaFree(d_tmp));
-#undef GEN_CUDA
-  (void)vbits;
-  rc = finish_layout(g);
-  if (rc) return fail(rc);
+  LUXB_CUDA(cudaGetLastError());
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  for (void* q : {(void*)d_keys, (void*)d_keys_alt, (void*)d_cursor}) tmp.release(q);
+  return finish_layout(g);
+}
+
+static int open_generated(const GenSpec& spec, const luxb_config* cfg, luxb_graph** out) {
+  luxb_graph* g = nullptr;
+  int rc = graph_begin(cfg, spec.nv, spec.ne, &g);
+  if (!rc) rc = generate_slice(g, spec);
+  if (rc) { if (g) luxb_close(g); return rc; }
   *out = g;
   return 0;
 }
@@ -715,6 +753,8 @@ int luxb_p2p_export(luxb_graph* g, void* blob, size_t* blob_bytes) {
   return 0;
 }
 
+static void p2p_unmap(luxb_graph* g);
+
 int luxb_p2p_import(luxb_graph* g, const void* all_blobs, size_t blob_bytes_each) {
   LUXB_ARG(g && all_blobs, "NULL argument");
   LUXB_ARG(blob_bytes_each == sizeof(P2PBlob), "blob size mismatch");
@@ -723,17 +763,7 @@ int luxb_p2p_import(luxb_graph* g, const void* all_blobs, size_t blob_bytes_each
   LUXB_ARG(g->comm != nullptr, "P2P exchange still needs the communicator for its iteration barrier");
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
   const P2PBlob* blobs = reinterpret_cast<const P2PBlob*>(all_blobs);
-  auto undo = [&]() {  // an import that fails half-way leaves nothing mapped
-    for (int p = 0; p < g->P; ++p) {
-      if (p == g->cfg.rank) continue;
-      for (int k = 0; k < 2; ++k) {
-        if (g->peer_val[k][p]) { cudaIpcCloseMemHandle(g->peer_val[k][p]); g->peer_val[k][p] = nullptr; }
-        if (g->peer_xt[k][p]) { cudaIpcCloseMemHandle(g->peer_xt[k][p]); g->peer_xt[k][p] = nullptr; }
-      }
-      if (g->peer_fq[p]) { cudaIpcCloseMemHandle(g->peer_fq[p]); g->peer_fq[p] = nullptr; }
-      if (g->peer_flags[p]) { cudaIpcCloseMemHandle(g->peer_flags[p]); g->peer_flags[p] = nullptr; }
-    }
-  };
+  // an import that fails half-way leaves nothing mapped (p2p_unmap)
   bool all_flags = g->flag_barrier && g->d_flags;
   for (int p = 0; p < g->P; ++p) all_flags = all_flags && (p == g->cfg.rank || blobs[p].has_flags);
   for (int p = 0; p < g->P; ++p) {
@@ -747,7 +777,7 @@ int luxb_p2p_import(luxb_graph* g, const void* all_blobs, size_t blob_bytes_each
       cudaError_t e = cudaIpcOpenMemHandle(&g->peer_flags[p], blobs[p].flags, cudaIpcMemLazyEnablePeerAccess);
       if (e != cudaSuccess) {
         set_error("cudaIpcOpenMemHandle (rank %d's barrier flags): %s", p, cudaGetErrorString(e));
-        undo();
+        p2p_unmap(g);
         return LUXB_ERR_CUDA;
       }
     }
@@ -755,7 +785,7 @@ int luxb_p2p_import(luxb_graph* g, const void* all_blobs, size_t blob_bytes_each
       cudaError_t e = cudaIpcOpenMemHandle(&g->peer_fq[p], blobs[p].fq, cudaIpcMemLazyEnablePeerAccess);
       if (e != cudaSuccess) {
         set_error("cudaIpcOpenMemHandle (rank %d's frontier slots): %s", p, cudaGetErrorString(e));
-        undo();
+        p2p_unmap(g);
         return LUXB_ERR_CUDA;
       }
     }
@@ -766,7 +796,7 @@ int luxb_p2p_import(luxb_graph* g, const void* all_blobs, size_t blob_bytes_each
         e = cudaIpcOpenMemHandle(&g->peer_xt[k][p], blobs[p].xt[k], cudaIpcMemLazyEnablePeerAccess);
       if (e != cudaSuccess) {
         set_error("cudaIpcOpenMemHandle (rank %d's buffers): %s", p, cudaGetErrorString(e));
-        undo();
+        p2p_unmap(g);
         return LUXB_ERR_CUDA;
       }
     }
@@ -806,27 +836,6 @@ int luxb_p2p_disconnect(luxb_graph* g) {
 }
 
 // ---- init ---------------------------------------------------------------------------------------------------
-extern "C++" {
-// temporaries of a build step: freed on every exit path
-struct DevTmp {
-  std::vector<void*> ptrs;
-  ~DevTmp() { for (void* q : ptrs) cudaFree(q); }
-  template <class T>
-  int alloc(T** out, uint64_t count) {
-    LUXB_TRY(dmalloc(out, count));
-    ptrs.push_back(*out);
-    return 0;
-  }
-  void release(void* q) {
-    for (size_t i = 0; i < ptrs.size(); ++i)
-      if (ptrs[i] == q) { cudaFree(q); ptrs.erase(ptrs.begin() + i); return; }
-  }
-  void keep(void* q) {  // ownership moves to the graph
-    for (size_t i = 0; i < ptrs.size(); ++i)
-      if (ptrs[i] == q) { ptrs.erase(ptrs.begin() + i); return; }
-  }
-};
-}  // extern "C++"
 static int build_push_csr(luxb_graph* g) {
   // CSR-by-source over this partition's own edges (init_push_* kernels, components_gpu.cu:550-607):
   // stable radix sort of (src, dst) pairs by src keeps each source's destinations ascending -> deterministic.
@@ -839,13 +848,9 @@ static int build_push_csr(luxb_graph* g) {
   const int grid = g->num_sms * 8;
   hist_src_kernel<<<grid, 256, 0, g->stream>>>(g->d_src, g->e_part, d_cnt);
   widen_u32_to_u64_kernel<<<grid, 256, 0, g->stream>>>(d_cnt, g->d_out_end, g->nv);
-  size_t tmp_bytes = 0;
-  LUXB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, g->d_out_end, g->d_out_end, (int)g->nv, g->stream));
-  void* d_tmp = nullptr;
-  LUXB_TRY(tmp.alloc((char**)&d_tmp, tmp_bytes + 256));
-  LUXB_CUDA(cub::DeviceScan::InclusiveSum(d_tmp, tmp_bytes, g->d_out_end, g->d_out_end, (int)g->nv, g->stream));
-  LUXB_CUDA(cudaStreamSynchronize(g->stream));
-  tmp.release(d_tmp);
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceScan::InclusiveSum(t, b, g->d_out_end, g->d_out_end, (int)g->nv, g->stream);
+  }));
   tmp.release(d_cnt);
   if (g->e_part == 0) return 0;
   uint32_t *d_dst = nullptr, *d_keys_out = nullptr;
@@ -855,28 +860,17 @@ static int build_push_csr(luxb_graph* g) {
   LUXB_CUDA(cudaGetLastError());
   int vbits = 1;
   while ((1ull << vbits) < (uint64_t)g->nv) ++vbits;
-  tmp_bytes = 0;
-  LUXB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, g->d_src, d_keys_out, d_dst, g->d_out_dst, (long long)g->e_part, 0,
-                                            vbits, g->stream));
-  LUXB_TRY(tmp.alloc((char**)&d_tmp, tmp_bytes + 256));
-  LUXB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, g->d_src, d_keys_out, d_dst, g->d_out_dst, (long long)g->e_part, 0,
-                                            vbits, g->stream));
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortPairs(t, b, g->d_src, d_keys_out, d_dst, g->d_out_dst, (long long)g->e_part, 0, vbits, g->stream);
+  }));
   if (g->cfg.app == LUXB_SSSP_WEIGHTED) {
     // the weights in the same order: the same stable sort on the same keys applies the same permutation
     LUXB_TRY(dmalloc(&g->d_out_w, g->e_part));
-    size_t w_bytes = 0;
-    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, w_bytes, g->d_src, d_keys_out, g->d_weight, g->d_out_w, (long long)g->e_part, 0,
-                                              vbits, g->stream));
-    if (w_bytes > tmp_bytes) {
-      LUXB_CUDA(cudaStreamSynchronize(g->stream));
-      tmp.release(d_tmp);
-      LUXB_TRY(tmp.alloc((char**)&d_tmp, w_bytes + 256));
-      tmp_bytes = w_bytes;
-    }
-    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, g->d_src, d_keys_out, g->d_weight, g->d_out_w, (long long)g->e_part, 0,
-                                              vbits, g->stream));
+    LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+      return cub::DeviceRadixSort::SortPairs(t, b, g->d_src, d_keys_out, g->d_weight, g->d_out_w, (long long)g->e_part, 0, vbits,
+                                             g->stream);
+    }));
   }
-  LUXB_CUDA(cudaStreamSynchronize(g->stream));
   return 0;
 }
 
@@ -1027,23 +1021,17 @@ static int build_hot_layout(luxb_graph* g, bool compact_cold) {
   hot_select_kernel<<<grid, 256, 0, g->stream>>>(g->d_deg, g->nv, tau, pt, d_cursor, d_cursor + 1, d_keys, d_ids, H);
   LUXB_CUDA(cudaGetLastError());
   // ids arrive in nondeterministic order: sort by (key, id) = two stable passes (id first, then key)
-  size_t tb = 0;
-  void* d_tmp = nullptr;
   int vbits = 1;
   while ((1ull << vbits) < (uint64_t)g->nv) ++vbits;
-  LUXB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_ids, d_ids2, d_keys, d_keys2, (int)H, 0, vbits, g->stream));
-  LUXB_TRY(tmp.alloc((char**)&d_tmp, tb + 256));
-  LUXB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, d_ids, d_ids2, d_keys, d_keys2, (int)H, 0, vbits, g->stream));
-  LUXB_CUDA(cudaStreamSynchronize(g->stream));
-  tmp.release(d_tmp);
-  tb = 0;
-  LUXB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_keys2, d_keys, d_ids2, g->d_hot_order, (int)H, 0, 32, g->stream));
-  LUXB_TRY(tmp.alloc((char**)&d_tmp, tb + 256));
-  LUXB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, d_keys2, d_keys, d_ids2, g->d_hot_order, (int)H, 0, 32, g->stream));
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortPairs(t, b, d_ids, d_ids2, d_keys, d_keys2, (int)H, 0, vbits, g->stream);
+  }));
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortPairs(t, b, d_keys2, d_keys, d_ids2, g->d_hot_order, (int)H, 0, 32, g->stream);
+  }));
   unsigned int h_cnt[1 + LUXB_MAX_PARTS];
   LUXB_CUDA(cudaMemcpyAsync(h_cnt, d_cursor, sizeof(h_cnt), cudaMemcpyDeviceToHost, g->stream));
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
-  tmp.release(d_tmp);
   g->hot_off[0] = 0;
   for (int p = 0; p < g->P; ++p) g->hot_off[p + 1] = g->hot_off[p] + h_cnt[1 + p];
   LUXB_TRY(tmp.alloc(&d_map, g->nv));
@@ -1054,16 +1042,14 @@ static int build_hot_layout(luxb_graph* g, bool compact_cold) {
     LUXB_TRY(tmp.alloc(&d_crank, (uint64_t)g->nv + 1));
     cold_flag_kernel<<<grid, 256, 0, g->stream>>>(g->d_deg, g->nv, tau, d_cflag);
     LUXB_CUDA(cudaMemsetAsync(d_cflag + g->nv, 0, 4, g->stream));
-    tb = 0;
-    LUXB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, d_cflag, d_crank, (int)g->nv + 1, g->stream));
-    LUXB_TRY(tmp.alloc((char**)&d_tmp, tb + 256));
-    LUXB_CUDA(cub::DeviceScan::ExclusiveSum(d_tmp, tb, d_cflag, d_crank, (int)g->nv + 1, g->stream));
+    LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+      return cub::DeviceScan::ExclusiveSum(t, b, d_cflag, d_crank, (int)g->nv + 1, g->stream);
+    }));
     for (int p = 0; p <= g->P; ++p) {
       const uint32_t at = p < g->P ? std::min(g->rl[p], g->nv) : g->nv;  // empty partitions sit at nv
       LUXB_CUDA(cudaMemcpyAsync(&g->cold_off[p], d_crank + at, 4, cudaMemcpyDeviceToHost, g->stream));
     }
     LUXB_CUDA(cudaStreamSynchronize(g->stream));
-    tmp.release(d_tmp);
     g->cold_n = g->cold_off[g->P];
     gather_map_compact_kernel<<<grid, 256, 0, g->stream>>>(d_map, d_crank, g->nv, H);
   } else {
@@ -1089,10 +1075,9 @@ static int build_hot_layout(luxb_graph* g, bool compact_cold) {
     LUXB_TRY(dmalloc(&g->d_zperm, H));
     owner_keys_kernel<<<grid, 256, 0, g->stream>>>(g->d_hot_order, H, pt, d_okeys, d_ranks);
     LUXB_CUDA(cudaGetLastError());
-    tb = 0;
-    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_okeys, d_okeys2, d_ranks, g->d_zperm, (int)H, 0, 8, g->stream));
-    LUXB_TRY(tmp.alloc((char**)&d_tmp, tb + 256));
-    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, d_okeys, d_okeys2, d_ranks, g->d_zperm, (int)H, 0, 8, g->stream));
+    LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+      return cub::DeviceRadixSort::SortPairs(t, b, d_okeys, d_okeys2, d_ranks, g->d_zperm, (int)H, 0, 8, g->stream);
+    }));
     const int me = g->cfg.rank;
     const uint32_t nh_me = g->hot_off[me + 1] - g->hot_off[me], nc_me = g->cold_off[me + 1] - g->cold_off[me];
     LUXB_TRY(dmalloc(&g->d_pack_list, (uint64_t)nh_me + nc_me + 1));
@@ -1102,8 +1087,6 @@ static int build_hot_layout(luxb_graph* g, bool compact_cold) {
     if (g->n_part)
       pack_list_cold_kernel<<<grid, 256, 0, g->stream>>>(d_cflag, d_crank, g->row_left, g->n_part, g->cold_off[me], g->d_pack_list + nh_me);
     LUXB_CUDA(cudaGetLastError());
-    LUXB_CUDA(cudaStreamSynchronize(g->stream));
-    tmp.release(d_tmp);
     g->packed = true;
   }
   gather_map_hot_kernel<<<grid, 256, 0, g->stream>>>(d_map, g->d_hot_order, H);
@@ -1121,6 +1104,26 @@ static int build_seg_sweep(luxb_graph* g);
 static int pagerank_publish(luxb_graph* g, float* x_new);
 static int wait_cold_exchange(luxb_graph* g);
 
+// The gather side of the pull sweeps: global out-degrees, the hot set (build_hot_layout), the flagged streams if
+// `streams` (build_seg_sweep) and the hot copies Z = [hot | compact cold values on one rank] + one whole table of slack:
+// the panel kernel always bulk-loads full blocks (panel.cuh); only the hot prefix gets the persisting window
+static int build_gather_side(luxb_graph* g, bool compact_cold, bool streams) {
+  LUXB_TRY(dmalloc(&g->d_deg, g->nv));
+  LUXB_CUDA(cudaMemsetAsync(g->d_deg, 0, (size_t)g->nv * 4, g->stream));
+  hist_src_kernel<<<g->num_sms * 8, 256, 0, g->stream>>>(g->d_src, g->e_part, g->d_deg);  // pull_scan_task_impl
+  LUXB_CUDA(cudaGetLastError());
+  if (g->P > 1) LUXB_NCCL(nccl().AllReduce(g->d_deg, g->d_deg, g->nv, ncclUint32, ncclSum, g->comm, g->stream));
+  LUXB_TRY(build_hot_layout(g, compact_cold));
+  if (streams) LUXB_TRY(build_seg_sweep(g));
+  if (g->hot_n) {
+    const uint64_t z_len = (uint64_t)g->hot_n + (g->cold_z ? g->cold_n : 0) + 65536;
+    LUXB_TRY(dmalloc((uint32_t**)&g->d_hot, z_len));
+    LUXB_CUDA(cudaMemsetAsync(g->d_hot, 0, z_len * 4, g->stream));
+    LUXB_TRY(set_l2_persisting_window(g, g->d_hot, (size_t)g->hot_n * 4));
+  }
+  return 0;
+}
+
 int luxb_init(luxb_graph* g) {
   LUXB_ARG(g != nullptr, "graph is NULL");
   if (g->inited) { set_error("luxb_init called twice"); return LUXB_ERR_STATE; }
@@ -1130,24 +1133,10 @@ int luxb_init(luxb_graph* g) {
   switch (g->cfg.app) {
     case LUXB_PAGERANK: {
       g->vbytes = 4;
-      LUXB_TRY(dmalloc(&g->d_deg, g->nv));
-      LUXB_CUDA(cudaMemsetAsync(g->d_deg, 0, (size_t)g->nv * 4, g->stream));
-      hist_src_kernel<<<grid, 256, 0, g->stream>>>(g->d_src, g->e_part, g->d_deg);  // pull_scan_task_impl
-      LUXB_CUDA(cudaGetLastError());
-      if (g->P > 1) LUXB_NCCL(nccl().AllReduce(g->d_deg, g->d_deg, g->nv, ncclUint32, ncclSum, g->comm, g->stream));
-      LUXB_TRY(build_hot_layout(g, /*compact_cold=*/true));
-      LUXB_TRY(build_seg_sweep(g));
+      LUXB_TRY(build_gather_side(g, /*compact_cold=*/true, /*streams=*/true));
       for (int k = 0; k < 2; ++k) LUXB_TRY(dmalloc((float**)&g->d_val[k], (uint64_t)g->nv + 64));
       pr_init_kernel<<<grid, 256, 0, g->stream>>>(g->d_deg, g->nv, (float*)g->d_val[0]);
       LUXB_CUDA(cudaMemsetAsync(g->d_val[1], 0, (size_t)g->nv * 4, g->stream));
-      if (g->hot_n) {
-        // + the compact cold values on one rank (Z = [hot | cold]) + one whole table of slack: the panel kernel always
-        // bulk-loads full blocks (panel.cuh); only the hot prefix gets the persisting window
-        const uint64_t z_len = (uint64_t)g->hot_n + (g->cold_z ? g->cold_n : 0) + 65536;
-        LUXB_TRY(dmalloc((float**)&g->d_hot, z_len));
-        LUXB_CUDA(cudaMemsetAsync(g->d_hot, 0, z_len * 4, g->stream));
-        LUXB_TRY(set_l2_persisting_window(g, g->d_hot, (size_t)g->hot_n * 4));
-      }
       if (g->packed) {
         g->xt_hot_chunk = ((((uint64_t)g->hot_n + g->P - 1) / g->P) + 31) & ~31ull;
         g->xt_cold_chunk = ((((uint64_t)g->cold_n + g->P - 1) / g->P) + 31) & ~31ull;
@@ -1169,20 +1158,18 @@ int luxb_init(luxb_graph* g) {
       cf_init_kernel<<<grid, 256, 0, g->stream>>>((float*)g->d_val[0], (uint64_t)g->nv * kCfK);
       cf_init_kernel<<<grid, 256, 0, g->stream>>>((float*)g->d_val[1], (uint64_t)g->nv * kCfK);
       // chunk table
+      DevTmp tmp;
       uint32_t* d_cnt = nullptr;
-      LUXB_TRY(dmalloc(&d_cnt, (uint64_t)g->n_part + 1));
+      LUXB_TRY(tmp.alloc(&d_cnt, (uint64_t)g->n_part + 1));
       LUXB_TRY(dmalloc(&g->d_chunk_first, (uint64_t)g->n_part + 2));
       LUXB_CUDA(cudaMemsetAsync(d_cnt, 0, ((size_t)g->n_part + 1) * 4, g->stream));
       cf_chunk_count_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, g->n_part, d_cnt);
-      size_t tmp_bytes = 0;
-      LUXB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_cnt, g->d_chunk_first, (int)g->n_part + 1, g->stream));
-      void* d_tmp = nullptr;
-      LUXB_CUDA(cudaMalloc(&d_tmp, tmp_bytes + 256));
-      LUXB_CUDA(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_cnt, g->d_chunk_first, (int)g->n_part + 1, g->stream));
+      LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+        return cub::DeviceScan::ExclusiveSum(t, b, d_cnt, g->d_chunk_first, (int)g->n_part + 1, g->stream);
+      }));
       LUXB_CUDA(cudaMemcpyAsync(&g->n_chunks, g->d_chunk_first + g->n_part, 4, cudaMemcpyDeviceToHost, g->stream));
       LUXB_CUDA(cudaStreamSynchronize(g->stream));
-      LUXB_CUDA(cudaFree(d_tmp));
-      LUXB_CUDA(cudaFree(d_cnt));
+      tmp.release(d_cnt);
       LUXB_TRY(dmalloc(&g->d_chunk_vtx, g->n_chunks));
       LUXB_TRY(dmalloc(&g->d_partial, (uint64_t)g->n_chunks * kCfK));
       cf_chunk_fill_kernel<<<grid, 256, 0, g->stream>>>(g->d_chunk_first, g->n_part, g->d_chunk_vtx);
@@ -1197,21 +1184,9 @@ int luxb_init(luxb_graph* g) {
       LUXB_TRY(dmalloc((uint32_t**)&g->d_val[0], g->nv));
       LUXB_TRY(dmalloc(&g->d_cur, g->n_part));
       LUXB_TRY(build_push_csr(g));
-      {  // hot-packed label copies for the pull sweeps (same layout as PageRank; refreshed before every pull sweep)
-        LUXB_TRY(dmalloc(&g->d_deg, g->nv));
-        LUXB_CUDA(cudaMemsetAsync(g->d_deg, 0, (size_t)g->nv * 4, g->stream));
-        hist_src_kernel<<<grid, 256, 0, g->stream>>>(g->d_src, g->e_part, g->d_deg);
-        LUXB_CUDA(cudaGetLastError());
-        if (g->P > 1) LUXB_NCCL(nccl().AllReduce(g->d_deg, g->d_deg, g->nv, ncclUint32, ncclSum, g->comm, g->stream));
-        LUXB_TRY(build_hot_layout(g, /*compact_cold=*/false));
-        // weighted SSSP pulls through the merge-path sweep only: the flagged streams carry no weights
-        if (g->cfg.app != LUXB_SSSP_WEIGHTED) LUXB_TRY(build_seg_sweep(g));
-        if (g->hot_n) {
-          LUXB_TRY(dmalloc((uint32_t**)&g->d_hot, (uint64_t)g->hot_n + 65536));  // + one table of slack (panel.cuh)
-          LUXB_CUDA(cudaMemsetAsync(g->d_hot, 0, ((size_t)g->hot_n + 65536) * 4, g->stream));
-          LUXB_TRY(set_l2_persisting_window(g, g->d_hot, (size_t)g->hot_n * 4));
-        }
-      }
+      // hot-packed label copies for the pull sweeps (same layout as PageRank; refreshed before every pull sweep).
+      // Weighted SSSP pulls through the merge-path sweep only: the flagged streams carry no weights.
+      LUXB_TRY(build_gather_side(g, /*compact_cold=*/false, /*streams=*/g->cfg.app != LUXB_SSSP_WEIGHTED));
       g->big_capacity = (uint32_t)std::min<uint64_t>(g->e_part / kPushBigDegree + 1024, 0x7FFFFFFFull);
       LUXB_TRY(dmalloc((PushArgs::BigSeg**)&g->d_big_list, g->big_capacity));
       LUXB_TRY(dmalloc(&g->d_fq_all, g->fq_total));
@@ -1277,26 +1252,6 @@ static int p2p_barrier(luxb_graph* g) {
 }
 
 extern "C++" {
-// the partition's own CSC as a layout view (it owns nothing but the fused fix-up's chain state)
-static PullLayout& base_layout(luxb_graph* g, const uint32_t* src_idx) {
-  PullLayout& L = g->base_view;
-  L.d_row_end = g->d_row_end;
-  L.d_row_end32 = g->d_row_end32;
-  L.d_src = const_cast<uint32_t*>(src_idx);
-  L.d_tile_v = g->d_tile_v;
-  L.n_vtx = g->n_part;
-  L.e_cnt = g->e_part;
-  L.n_tiles = g->n_tiles;
-  L.d_head = g->d_head;
-  L.d_tail = g->d_tail;
-  L.d_carry = g->d_carry;
-  L.d_carry_flag = g->d_carry_flag;
-  L.d_block_agg = g->d_block_agg;
-  L.d_block_flag = g->d_block_flag;
-  L.n_fix_blocks = g->n_fix_blocks;
-  return L;
-}
-
 template <class Prog, class Shape>
 static int launch_pull_shape(luxb_graph* g, const PullArgs<Prog>& a) {
   auto kern = pull_tile_kernel<Prog, Shape>;
@@ -1334,60 +1289,60 @@ static int kt_end(luxb_graph* g) {
 }
 
 template <class Prog>
-static void fill_fixup_args(PullArgs<Prog>& a, const PullLayout& L) {
-  a.tile_v = L.d_tile_v;
-  a.n_tiles = L.n_tiles;
-  a.head_partial = reinterpret_cast<typename Prog::Acc*>(L.d_head);
-  a.tail_partial = reinterpret_cast<typename Prog::Acc*>(L.d_tail);
-  a.carry = reinterpret_cast<typename Prog::Wide*>(L.d_carry);
-  a.carry_flag = L.d_carry_flag;
-  a.block_agg = reinterpret_cast<typename Prog::Wide*>(L.d_block_agg);
-  a.block_flag = L.d_block_flag;
+static void fill_fixup_args(PullArgs<Prog>& a, const FixupScratch& f) {
+  a.head_partial = reinterpret_cast<typename Prog::Acc*>(f.d_head);
+  a.tail_partial = reinterpret_cast<typename Prog::Acc*>(f.d_tail);
+  a.carry = reinterpret_cast<typename Prog::Wide*>(f.d_carry);
+  a.carry_flag = f.d_carry_flag;
+  a.block_agg = reinterpret_cast<typename Prog::Wide*>(f.d_block_agg);
+  a.block_flag = f.d_block_flag;
 }
 
-// L is the layout's own descriptor (the fused fix-up keeps its launch epoch there)
+// f is the sweep's own scratch (the fused fix-up keeps its launch epoch there)
 template <class Prog>
-static int launch_fixup(luxb_graph* g, const PullArgs<Prog>& a, PullLayout& L) {
-  if (L.n_tiles <= 1) return 0;
+static int launch_fixup(luxb_graph* g, const PullArgs<Prog>& a, FixupScratch& f) {
+  if (a.n_tiles <= 1) return 0;
   if (g->fused_fixup) {
-    if (!L.d_chain) {
-      LUXB_TRY(dmalloc(&L.d_chain, 4ull * L.n_fix_blocks + 4));  // values, status words, [4 n] = ticket counter
-      LUXB_CUDA(cudaMemsetAsync(L.d_chain, 0, (4ull * L.n_fix_blocks + 4) * 8, g->stream));
-      L.chain_epoch = 0;
+    if (!f.d_chain) {
+      LUXB_TRY(dmalloc(&f.d_chain, 4ull * f.n_fix_blocks + 4));  // values, status words, [4 n] = ticket counter
+      LUXB_CUDA(cudaMemsetAsync(f.d_chain, 0, (4ull * f.n_fix_blocks + 4) * 8, g->stream));
+      f.chain_epoch = 0;
     }
     FixupChain<Prog> ch;
-    ch.value = L.d_chain;
-    ch.status = L.d_chain + 2ull * L.n_fix_blocks;
-    ch.ticket = L.d_chain + 4ull * L.n_fix_blocks;
-    ch.n_blocks = L.n_fix_blocks;
-    ch.epoch = ++L.chain_epoch;
-    if (L.chain_epoch >= 0x3FFFFFF0u) {  // 30-bit epochs: start over with a clean status array
-      LUXB_CUDA(cudaMemsetAsync(L.d_chain, 0, (4ull * L.n_fix_blocks + 4) * 8, g->stream));
-      L.chain_epoch = ch.epoch = 1;
+    ch.value = f.d_chain;
+    ch.status = f.d_chain + 2ull * f.n_fix_blocks;
+    ch.ticket = f.d_chain + 4ull * f.n_fix_blocks;
+    ch.n_blocks = f.n_fix_blocks;
+    ch.epoch = ++f.chain_epoch;
+    if (f.chain_epoch >= 0x3FFFFFF0u) {  // 30-bit epochs: start over with a clean status array
+      LUXB_CUDA(cudaMemsetAsync(f.d_chain, 0, (4ull * f.n_fix_blocks + 4) * 8, g->stream));
+      f.chain_epoch = ch.epoch = 1;
     }
-    pull_fixup_fused_kernel<Prog><<<L.n_fix_blocks, kFixBlock, 0, g->stream>>>(a, ch);
+    pull_fixup_fused_kernel<Prog><<<f.n_fix_blocks, kFixBlock, 0, g->stream>>>(a, ch);
     LUXB_CUDA(cudaGetLastError());
     g->stats.kernel_launches++;
     return 0;
   }
-  pull_fixup_scan_kernel<Prog><<<L.n_fix_blocks, kFixBlock, 0, g->stream>>>(a);
-  pull_fixup_blocks_kernel<Prog><<<1, 1024, 0, g->stream>>>(a, L.n_fix_blocks);
-  pull_fixup_apply_kernel<Prog><<<L.n_fix_blocks, kFixBlock, 0, g->stream>>>(a);
+  pull_fixup_scan_kernel<Prog><<<f.n_fix_blocks, kFixBlock, 0, g->stream>>>(a);
+  pull_fixup_blocks_kernel<Prog><<<1, 1024, 0, g->stream>>>(a, f.n_fix_blocks);
+  pull_fixup_apply_kernel<Prog><<<f.n_fix_blocks, kFixBlock, 0, g->stream>>>(a);
   LUXB_CUDA(cudaGetLastError());
   g->stats.kernel_launches += 3;
   return 0;
 }
 
-// one pull sweep over layout L.  hub_bits != nullptr: those vertices get their raw sum (panel.cuh).
+// one pull sweep over layout L gathering through the ids `src`.  hub_bits != nullptr: those vertices get their raw sum
+// (panel.cuh).
 template <class Prog>
-static int launch_pull(luxb_graph* g, PullLayout& L, const typename Prog::Vertex* x_nat, const typename Prog::Vertex* x_cold,
-                       const typename Prog::Vertex* x_hot, uint32_t hot_n, typename Prog::Vertex* out_local,
-                       const typename Prog::Params& prm, const uint32_t* hub_bits = nullptr, bool timed = true) {
+static int launch_pull(luxb_graph* g, PullLayout& L, const uint32_t* src, const typename Prog::Vertex* x_nat,
+                       const typename Prog::Vertex* x_cold, const typename Prog::Vertex* x_hot, uint32_t hot_n,
+                       typename Prog::Vertex* out_local, const typename Prog::Params& prm, const uint32_t* hub_bits = nullptr,
+                       bool timed = true) {
   if (L.n_tiles == 0) return 0;
   PullArgs<Prog> a{};
   a.row_end = L.d_row_end;
   a.row_end32 = L.d_row_end32;
-  a.src = reinterpret_cast<const uint32_t*>(L.d_src);
+  a.src = src;
   a.x_nat = x_nat;
   a.n_part = L.n_vtx;
   a.e_part = L.e_cnt;
@@ -1396,13 +1351,15 @@ static int launch_pull(luxb_graph* g, PullLayout& L, const typename Prog::Vertex
   a.x_hot = x_hot;
   a.hot_n = hot_n;
   a.out = out_local;
-  fill_fixup_args(a, L);
+  a.tile_v = L.d_tile_v;
+  a.n_tiles = L.n_tiles;
+  fill_fixup_args(a, L.fix);
   a.tile_counter = reinterpret_cast<uint32_t*>(g->d_counters + 2);
   LUXB_CUDA(cudaMemsetAsync(a.tile_counter, 0, 4, g->stream));
   a.prm = prm;
   a.hub_bits = hub_bits;
   a.raw_out = 0;
-  if constexpr (Prog::kWeighted) a.weight = g->d_weight;  // CSC order = the order of L.d_src (base layout only)
+  if constexpr (Prog::kWeighted) a.weight = g->d_weight;  // CSC order = the order of src (base layout only)
   if (timed) LUXB_TRY(kt_begin(g));
   switch (g->pull_shape) {
 #define LUXB_CASE_SHAPE(id, ipt, warps, stages) \
@@ -1413,7 +1370,7 @@ static int launch_pull(luxb_graph* g, PullLayout& L, const typename Prog::Vertex
   if (timed) LUXB_TRY(kt_end(g));
   g->stats.kernel_launches++;
   pt_mark(g, 0);
-  LUXB_TRY(launch_fixup(g, a, L));
+  LUXB_TRY(launch_fixup(g, a, L.fix));
   pt_mark(g, 1);
   return 0;
 }
@@ -1438,10 +1395,12 @@ static const SegShapeInfo kSegPanelInfo[] = {LUXB_SEG_PANEL_SHAPES(LUXB_PSHAPE_I
 static const int kNumSegMain = sizeof(kSegMainInfo) / sizeof(SegShapeInfo);
 static const int kNumSegPanel = sizeof(kSegPanelInfo) / sizeof(SegShapeInfo);
 
-static void free_layout(PullLayout& L) {
-  void* ptrs[] = {L.d_row_end, L.d_row_end32, L.d_src, L.d_tile_v, L.d_head, L.d_tail, L.d_carry, L.d_carry_flag, L.d_block_agg, L.d_block_flag,
-                  L.d_close, L.d_empty, L.d_empty_hub, L.d_chain};
+// owns_csc = false: L.d_row_end and L.d_src belong to the graph (the base layout)
+static void free_layout(PullLayout& L, bool owns_csc = true) {
+  void* ptrs[] = {owns_csc ? L.d_row_end : nullptr, L.d_row_end32, owns_csc ? L.d_src : nullptr, L.d_tile_v, L.d_close, L.d_empty,
+                  L.d_empty_hub};
   for (void* q : ptrs) if (q) cudaFree(q);
+  free_fixup(L.fix);
   L = PullLayout();
 }
 
@@ -1487,15 +1446,12 @@ static int build_seg_stream(luxb_graph* g, PullLayout& L, const uint64_t* d_row_
   LUXB_TRY(tmp.alloc(&d_rank, (uint64_t)n_vtx + 1));
   nonempty_flag_kernel<<<grid, 256, 0, g->stream>>>(d_row_end, n_vtx, d_flag);
   LUXB_CUDA(cudaMemsetAsync(d_flag + n_vtx, 0, 4, g->stream));
-  size_t tb = 0;
-  void* d_tmp = nullptr;
-  LUXB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, d_flag, d_rank, (int)n_vtx + 1, g->stream));
-  LUXB_TRY(tmp.alloc((char**)&d_tmp, tb + 256));
-  LUXB_CUDA(cub::DeviceScan::ExclusiveSum(d_tmp, tb, d_flag, d_rank, (int)n_vtx + 1, g->stream));
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceScan::ExclusiveSum(t, b, d_flag, d_rank, (int)n_vtx + 1, g->stream);
+  }));
   uint32_t n_seg = 0;
   LUXB_CUDA(cudaMemcpyAsync(&n_seg, d_rank + n_vtx, 4, cudaMemcpyDeviceToHost, g->stream));
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
-  tmp.release(d_tmp);
   // 2. words: ids, then pads, then head flags; close list (entry j + 1 = owner of head j, dummies for the pads)
   Word* d_words = nullptr;
   LUXB_TRY(dmalloc(&d_words, words + 64));
@@ -1519,10 +1475,9 @@ static int build_seg_stream(luxb_graph* g, PullLayout& L, const uint64_t* d_row_
   piece_heads_kernel<Word><<<grid, 256, 0, g->stream>>>(d_words, L.n_tiles, piece, d_cnt);
   LUXB_CUDA(cudaGetLastError());
   LUXB_TRY(dmalloc(&L.d_tile_v, (uint64_t)L.n_tiles + 2));
-  tb = 0;
-  LUXB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, d_cnt, L.d_tile_v, (int)L.n_tiles + 1, g->stream));
-  LUXB_TRY(tmp.alloc((char**)&d_tmp, tb + 256));
-  LUXB_CUDA(cub::DeviceScan::ExclusiveSum(d_tmp, tb, d_cnt, L.d_tile_v, (int)L.n_tiles + 1, g->stream));
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceScan::ExclusiveSum(t, b, d_cnt, L.d_tile_v, (int)L.n_tiles + 1, g->stream);
+  }));
   uint32_t heads_counted = 0;
   LUXB_CUDA(cudaMemcpyAsync(&heads_counted, L.d_tile_v + L.n_tiles, 4, cudaMemcpyDeviceToHost, g->stream));
   // 4. vertices without edges (hubs among them apart)
@@ -1547,14 +1502,7 @@ static int build_seg_stream(luxb_graph* g, PullLayout& L, const uint64_t* d_row_
     return LUXB_ERR_STATE;
   }
   // 5. fix-up scratch
-  LUXB_TRY(dmalloc((uint32_t**)&L.d_head, (uint64_t)L.n_tiles + 1));
-  LUXB_TRY(dmalloc((uint32_t**)&L.d_tail, (uint64_t)L.n_tiles + 1));
-  L.n_fix_blocks = (L.n_tiles + kFixBlock - 1) / kFixBlock;
-  LUXB_TRY(dmalloc((uint64_t**)&L.d_carry, (uint64_t)L.n_tiles + 1));
-  LUXB_TRY(dmalloc(&L.d_carry_flag, (uint64_t)L.n_tiles + 1));
-  LUXB_TRY(dmalloc((uint64_t**)&L.d_block_agg, (uint64_t)L.n_fix_blocks + 1));
-  LUXB_TRY(dmalloc(&L.d_block_flag, (uint64_t)L.n_fix_blocks + 1));
-  return 0;
+  return alloc_fixup(L.fix, L.n_tiles);
 }
 }  // extern "C++"
 
@@ -1604,16 +1552,13 @@ static int build_panel_layout(luxb_graph* g) {
   LUXB_TRY(tmp.alloc(&d_hub_idx, (uint64_t)g->n_part + 1));
   hub_flag_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, g->n_part, min_indeg, d_flag);
   LUXB_CUDA(cudaGetLastError());
-  size_t tb = 0;
-  void* d_scan_tmp = nullptr;
-  LUXB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, d_flag, d_hub_idx, (int)g->n_part, g->stream));
-  LUXB_TRY(tmp.alloc((char**)&d_scan_tmp, tb + 256));
-  LUXB_CUDA(cub::DeviceScan::ExclusiveSum(d_scan_tmp, tb, d_flag, d_hub_idx, (int)g->n_part, g->stream));
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceScan::ExclusiveSum(t, b, d_flag, d_hub_idx, (int)g->n_part, g->stream);
+  }));
   uint32_t last_idx = 0, last_flag = 0;
   LUXB_CUDA(cudaMemcpyAsync(&last_idx, d_hub_idx + g->n_part - 1, 4, cudaMemcpyDeviceToHost, g->stream));
   LUXB_CUDA(cudaMemcpyAsync(&last_flag, d_flag + g->n_part - 1, 4, cudaMemcpyDeviceToHost, g->stream));
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
-  tmp.release(d_scan_tmp);
   const uint32_t Nh = last_idx + last_flag;
   if (Nh == 0 || (uint64_t)Nh * NB0 >= 0x7FFFFFF0ull) return 0;
   uint32_t *d_hub_vtx = nullptr, *d_hub_bits = nullptr, *d_cov = nullptr;
@@ -1631,16 +1576,14 @@ static int build_panel_layout(luxb_graph* g) {
     LUXB_TRY(tmp.alloc(&d_hvtx2, Nh));
     hub_order_key_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, d_hub_vtx, Nh, d_hkey);
     LUXB_CUDA(cudaGetLastError());
-    tb = 0;
-    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_hkey, d_hkey2, d_hub_vtx, d_hvtx2, (int)Nh, 0, 32, g->stream));
-    LUXB_TRY(tmp.alloc((char**)&d_scan_tmp, tb + 256));
-    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(d_scan_tmp, tb, d_hkey, d_hkey2, d_hub_vtx, d_hvtx2, (int)Nh, 0, 32, g->stream));
+    LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+      return cub::DeviceRadixSort::SortPairs(t, b, d_hkey, d_hkey2, d_hub_vtx, d_hvtx2, (int)Nh, 0, 32, g->stream);
+    }));
     LUXB_CUDA(cudaMemcpyAsync(d_hub_vtx, d_hvtx2, (size_t)Nh * 4, cudaMemcpyDeviceToDevice, g->stream));
     hub_pos_kernel<<<grid, 256, 0, g->stream>>>(d_hub_vtx, Nh, d_hub_idx);
     LUXB_CUDA(cudaGetLastError());
     LUXB_CUDA(cudaMemcpyAsync(hub_key.data(), d_hkey2, (size_t)Nh * 4, cudaMemcpyDeviceToHost, g->stream));
     LUXB_CUDA(cudaStreamSynchronize(g->stream));
-    tmp.release(d_scan_tmp);
     tmp.release(d_hkey);
     tmp.release(d_hkey2);
     tmp.release(d_hvtx2);
@@ -1726,15 +1669,12 @@ static int build_panel_layout(luxb_graph* g) {
     cub::DoubleBuffer<uint64_t> pb(d_pay, d_pay2);
     int hbits = 1;
     while ((1ull << hbits) < (uint64_t)Nh) ++hbits;
-    size_t tb1 = 0, tb2 = 0;
-    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb1, pb, kb, (long long)g->e_part, 32, 32 + hbits, g->stream));
-    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb2, kb, pb, (long long)g->e_part, 0, kSplitKeyBits, g->stream));
-    tb = std::max(tb1, tb2);
-    LUXB_TRY(tmp.alloc((char**)&d_scan_tmp, tb + 256));
-    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(d_scan_tmp, tb, pb, kb, (long long)g->e_part, 32, 32 + hbits, g->stream));
-    LUXB_CUDA(cub::DeviceRadixSort::SortPairs(d_scan_tmp, tb, kb, pb, (long long)g->e_part, 0, kSplitKeyBits, g->stream));
-    LUXB_CUDA(cudaStreamSynchronize(g->stream));
-    tmp.release(d_scan_tmp);
+    LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+      return cub::DeviceRadixSort::SortPairs(t, b, pb, kb, (long long)g->e_part, 32, 32 + hbits, g->stream);
+    }));
+    LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+      return cub::DeviceRadixSort::SortPairs(t, b, kb, pb, (long long)g->e_part, 0, kSplitKeyBits, g->stream);
+    }));
     tmp.release(kb.Alternate());
     tmp.release(pb.Alternate());
     d_key2 = kb.Current();
@@ -1776,12 +1716,9 @@ static int build_panel_layout(luxb_graph* g) {
   LUXB_CUDA(cudaGetLastError());
   LUXB_TRY(tmp.alloc(&d_vrow, (uint64_t)NV + 4));
   widen_u32_to_u64_kernel<<<grid, 256, 0, g->stream>>>(d_vcount, d_vrow, NV);
-  tb = 0;
-  LUXB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb, d_vrow, d_vrow, (int)NV, g->stream));
-  LUXB_TRY(tmp.alloc((char**)&d_scan_tmp, tb + 256));
-  LUXB_CUDA(cub::DeviceScan::InclusiveSum(d_scan_tmp, tb, d_vrow, d_vrow, (int)NV, g->stream));
-  LUXB_CUDA(cudaStreamSynchronize(g->stream));
-  tmp.release(d_scan_tmp);
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceScan::InclusiveSum(t, b, d_vrow, d_vrow, (int)NV, g->stream);
+  }));
   tmp.release(d_vcount);
   LUXB_TRY((build_seg_stream<uint16_t, uint16_t>(g, g->sb_panel, d_vrow, NV, d_src16, e_cov, pblk, (uint32_t)shp.stage_edges,
                                                  (uint32_t)shp.piece, 0, false, nullptr, g->sb_super_end)));
@@ -1801,12 +1738,9 @@ static int build_panel_layout(luxb_graph* g) {
     LUXB_CUDA(cudaGetLastError());
     LUXB_TRY(tmp.alloc(&d_crow, (uint64_t)NVc + 4));
     widen_u32_to_u64_kernel<<<grid, 256, 0, g->stream>>>(d_ccount, d_crow, NVc);
-    tb = 0;
-    LUXB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb, d_crow, d_crow, (int)NVc, g->stream));
-    LUXB_TRY(tmp.alloc((char**)&d_scan_tmp, tb + 256));
-    LUXB_CUDA(cub::DeviceScan::InclusiveSum(d_scan_tmp, tb, d_crow, d_crow, (int)NVc, g->stream));
-    LUXB_CUDA(cudaStreamSynchronize(g->stream));
-    tmp.release(d_scan_tmp);
+    LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+      return cub::DeviceScan::InclusiveSum(t, b, d_crow, d_crow, (int)NVc, g->stream);
+    }));
     tmp.release(d_ccount);
     g->cs_shape = env_int("LUXB_CS_SHAPE", g->seg_main_shape);
     if (g->cs_shape < 0 || g->cs_shape >= kNumSegMain) g->cs_shape = 0;
@@ -1832,15 +1766,13 @@ static int build_panel_layout(luxb_graph* g) {
   LUXB_TRY(tmp.alloc(&d_main_row, (uint64_t)g->n_part + 4));
   main_indeg_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, g->n_part, d_flag, d_hub_idx, d_cov, S ? d_cold_cnt : nullptr, d_main_row);
   LUXB_CUDA(cudaGetLastError());
-  tb = 0;
-  LUXB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb, d_main_row, d_main_row, (int)g->n_part, g->stream));
-  LUXB_TRY(tmp.alloc((char**)&d_scan_tmp, tb + 256));
-  LUXB_CUDA(cub::DeviceScan::InclusiveSum(d_scan_tmp, tb, d_main_row, d_main_row, (int)g->n_part, g->stream));
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceScan::InclusiveSum(t, b, d_main_row, d_main_row, (int)g->n_part, g->stream);
+  }));
   uint64_t chk = 0;
   LUXB_CUDA(cudaMemcpyAsync(&chk, d_main_row + g->n_part - 1, 8, cudaMemcpyDeviceToHost, g->stream));
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
   if (chk != e_main) { set_error("panel split: offsets do not add up"); return LUXB_ERR_STATE; }
-  tmp.release(d_scan_tmp);
   tmp.release(d_key2);
   tmp.release(d_pay2);
   const SegShapeInfo mshp = kSegMainInfo[g->seg_main_shape];
@@ -1863,7 +1795,6 @@ static int build_panel_layout(luxb_graph* g) {
   g->sb_n_hub = Nh;
   g->sb_n_blocks = NB;
   g->sb_bs = bs;
-  g->sb_n_src = n_src;
   g->sb_on = true;
   g->cs_on = S > 0;
   g->cs_n_seg = S;
@@ -1922,12 +1853,38 @@ static int launch_seg_shape(luxb_graph* g, const SegArgs<Prog>& a, int ctas_per_
   return 0;
 }
 
-template <class Prog>
-static void fill_seg_args(SegArgs<Prog>& a, const PullLayout& L) {
-  fill_fixup_args(a.p, L);
+// one flagged stream L (seg.cuh): the seg kernel in shape `shape` of the panel (kPanel) or the main family, then its
+// fix-up.  The caller has set a's stream-specific fields; L's own arrays are filled here.  counter_slot: the stream's
+// tile counter in d_counters; tag: the phase-timer slot of the kernel.
+template <bool kPanel, class Prog>
+static int launch_seg_stream(luxb_graph* g, PullLayout& L, SegArgs<Prog>& a, int shape, int ctas_per_sm, int counter_slot, int tag,
+                             const char* name) {
+  a.p.tile_v = L.d_tile_v;
+  a.p.n_tiles = L.n_tiles;
+  fill_fixup_args(a.p, L.fix);
   a.p.close_vtx = L.d_close;
   a.words = L.d_src;
   a.n_stages = L.n_stages;
+  a.tile_counter = reinterpret_cast<uint32_t*>(g->d_counters + counter_slot);
+  LUXB_CUDA(cudaMemsetAsync(a.tile_counter, 0, 4, g->stream));
+#define LUXB_CASE_MSHAPE(id, warps, stages, rounds) \
+  case id: LUXB_TRY((launch_seg_shape<Prog, SegMain##id>(g, a, ctas_per_sm))); break;
+#define LUXB_CASE_PSHAPE(id, warps, stages, rounds, tab, v) \
+  case id: LUXB_TRY((launch_seg_shape<Prog, SegPanel##id>(g, a, ctas_per_sm))); break;
+  if constexpr (kPanel) {
+    switch (shape) {
+      LUXB_SEG_PANEL_SHAPES(LUXB_CASE_PSHAPE)
+      default: set_error("bad %s shape", name); return LUXB_ERR_STATE;
+    }
+  } else {
+    switch (shape) {
+      LUXB_SEG_MAIN_SHAPES(LUXB_CASE_MSHAPE)
+      default: set_error("bad %s shape", name); return LUXB_ERR_STATE;
+    }
+  }
+  g->stats.kernel_launches++;
+  pt_mark(g, tag);
+  return launch_fixup(g, a.p, L.fix);
 }
 }  // extern "C++"
 
@@ -1939,7 +1896,6 @@ template <class Prog>
 static int launch_seg_main(luxb_graph* g, PullLayout& L, const typename Prog::Vertex* x_nat, const typename Prog::Vertex* x_cold,
                            typename Prog::Vertex* out_local, int out_buffer, const typename Prog::Params& prm, const uint32_t* hub_bits) {
   SegArgs<Prog> a{};
-  fill_seg_args(a, L);
   a.p.n_part = L.n_vtx;
   a.p.row_left = g->row_left;
   a.p.x_nat = x_nat;
@@ -1951,17 +1907,7 @@ static int launch_seg_main(luxb_graph* g, PullLayout& L, const typename Prog::Ve
   a.p.hub_bits = hub_bits;
   a.p.l2_hints = g->l2_hints;
   LUXB_TRY(wait_cold_exchange(g));
-  a.tile_counter = reinterpret_cast<uint32_t*>(g->d_counters + 2);
-  LUXB_CUDA(cudaMemsetAsync(a.tile_counter, 0, 4, g->stream));
-  switch (g->seg_main_shape) {
-#define LUXB_CASE_MSHAPE(id, warps, stages, rounds) \
-    case id: LUXB_TRY((launch_seg_shape<Prog, SegMain##id>(g, a, g->pull_ctas))); break;
-    LUXB_SEG_MAIN_SHAPES(LUXB_CASE_MSHAPE)
-    default: set_error("bad seg shape"); return LUXB_ERR_STATE;
-  }
-  g->stats.kernel_launches++;
-  pt_mark(g, 0);
-  LUXB_TRY(launch_fixup(g, a.p, L));
+  LUXB_TRY((launch_seg_stream<false, Prog>(g, L, a, g->seg_main_shape, g->pull_ctas, 2, 0, "seg")));
   // vertices without in-edges in this stream.  PageRank: update(identity) is a constant -> written once per value
   // buffer.  Hubs among them need the raw identity every sweep (the combine overwrites it).
   if (out_buffer >= 0 && L.n_empty && !g->empties_done[out_buffer]) {
@@ -1985,9 +1931,7 @@ static int sweep_seg(luxb_graph* g, const typename Prog::Vertex* x_nat, const ty
   using Acc = typename Prog::Acc;
   LUXB_TRY(kt_begin(g));
   if (g->sb_on) {
-    PullLayout& PL = g->sb_panel;
     SegArgs<Prog> pa{};
-    fill_seg_args(pa, PL);
     pa.p.x_hot = reinterpret_cast<const typename Prog::Vertex*>(g->d_hot);
     pa.p.out = reinterpret_cast<typename Prog::Vertex*>(g->d_sb_partial);
     pa.p.raw_out = 1;
@@ -1995,25 +1939,13 @@ static int sweep_seg(luxb_graph* g, const typename Prog::Vertex* x_nat, const ty
     pa.bs = g->sb_bs;
     pa.n_blocks = g->sb_n_blocks;
     for (uint32_t b = 0; b < g->sb_n_blocks; ++b) pa.super_end[b] = g->sb_super_end[b];
-    pa.tile_counter = reinterpret_cast<uint32_t*>(g->d_counters + 4);
-    LUXB_CUDA(cudaMemsetAsync(pa.tile_counter, 0, 4, g->stream));
-    switch (g->seg_panel_shape) {
-#define LUXB_CASE_PSHAPE(id, warps, stages, rounds, tab, v) \
-      case id: LUXB_TRY((launch_seg_shape<Prog, SegPanel##id>(g, pa, 1))); break;
-      LUXB_SEG_PANEL_SHAPES(LUXB_CASE_PSHAPE)
-      default: set_error("bad panel shape"); return LUXB_ERR_STATE;
-    }
-    g->stats.kernel_launches++;
-    pt_mark(g, 5);
-    LUXB_TRY(launch_fixup(g, pa.p, PL));
+    LUXB_TRY((launch_seg_stream<true, Prog>(g, g->sb_panel, pa, g->seg_panel_shape, 1, 4, 5, "panel")));
     pt_mark(g, 1);
   }
   if (g->cs_on) {
     // cold-hub stream: raw partial per (cold segment, hub); its gathers all index the compact cold values, which it
     // loads with evict_normal (l2_hints = 0): the current segment is meant to stay in L2 while the SMs sweep it
-    PullLayout& CL = g->sb_cold;
     SegArgs<Prog> ca{};
-    fill_seg_args(ca, CL);
     ca.p.x_old = x_cold;
     ca.p.x_hot = reinterpret_cast<const typename Prog::Vertex*>(g->d_hot);
     ca.p.hot_n = g->hot_n;
@@ -2021,17 +1953,7 @@ static int sweep_seg(luxb_graph* g, const typename Prog::Vertex* x_nat, const ty
     ca.p.raw_out = 1;
     ca.p.l2_hints = 0;
     ca.p.prm = prm;
-    ca.tile_counter = reinterpret_cast<uint32_t*>(g->d_counters + 4);
-    LUXB_CUDA(cudaMemsetAsync(ca.tile_counter, 0, 4, g->stream));
-    switch (g->cs_shape) {
-#define LUXB_CASE_CSHAPE(id, warps, stages, rounds) \
-      case id: LUXB_TRY((launch_seg_shape<Prog, SegMain##id>(g, ca, g->pull_ctas))); break;
-      LUXB_SEG_MAIN_SHAPES(LUXB_CASE_CSHAPE)
-      default: set_error("bad cold-hub shape"); return LUXB_ERR_STATE;
-    }
-    g->stats.kernel_launches++;
-    pt_mark(g, 9);
-    LUXB_TRY(launch_fixup(g, ca.p, CL));
+    LUXB_TRY((launch_seg_stream<false, Prog>(g, g->sb_cold, ca, g->cs_shape, g->pull_ctas, 4, 9, "cold-hub")));
     pt_mark(g, 1);
   }
   LUXB_TRY((launch_seg_main<Prog>(g, g->sb_main, x_nat, x_cold, out_local, out_buffer, prm, g->sb_on ? g->d_hub_bits : nullptr)));
@@ -2190,7 +2112,7 @@ static int pagerank_iteration(luxb_graph* g) {
     LUXB_TRY((sweep_seg<PageRankProgram>(g, x_old, x_cold, x_new + g->row_left, 1 - g->cur, prm)));
   } else {
     LUXB_TRY(wait_cold_exchange(g));
-    LUXB_TRY(launch_pull<PageRankProgram>(g, base_layout(g, g->hot_n ? g->d_src_gather : g->d_src), x_old, x_cold, (const float*)g->d_hot,
+    LUXB_TRY(launch_pull<PageRankProgram>(g, g->base, g->hot_n ? g->d_src_gather : g->d_src, x_old, x_cold, (const float*)g->d_hot,
                                           g->hot_n, x_new + g->row_left, prm));
   }
   LUXB_TRY(pagerank_publish(g, x_new));
@@ -2269,7 +2191,7 @@ static int label_iteration(luxb_graph* g) {
       }
     }
     if (!swept)
-      LUXB_TRY(launch_pull<Prog>(g, base_layout(g, g->hot_n ? g->d_src_gather : g->d_src), lab, lab, (const uint32_t*)g->d_hot, g->hot_n,
+      LUXB_TRY(launch_pull<Prog>(g, g->base, g->hot_n ? g->d_src_gather : g->d_src, lab, lab, (const uint32_t*)g->d_hot, g->hot_n,
                                  g->d_cur, prm));
     g->stats.edges_processed += g->e_part;
     g->stats.pull_iterations++;
@@ -2704,7 +2626,7 @@ int luxb_debug_gather_ms(luxb_graph* g, int packed, float* ms_out) {
   float best = 1e30f;
   for (int r = 0; r < 4; ++r) {
     LUXB_CUDA(cudaEventRecord(g->ev_begin, g->stream));
-    debug_gather_kernel<<<g->num_sms * 4, 256, 0, g->stream>>>(idx, nat, (const float*)g->d_hot, hn, g->e_part, (float*)g->d_head);
+    debug_gather_kernel<<<g->num_sms * 4, 256, 0, g->stream>>>(idx, nat, (const float*)g->d_hot, hn, g->e_part, (float*)g->base.fix.d_head);
     LUXB_CUDA(cudaEventRecord(g->ev_end, g->stream));
     LUXB_CUDA(cudaStreamSynchronize(g->stream));
     float ms = 0.f;
@@ -2757,20 +2679,19 @@ void luxb_close(luxb_graph* g) {
   if (g->ev_cold) cudaEventDestroy(g->ev_cold);
   if (g->stream2) cudaStreamDestroy(g->stream2);
 
-  void* ptrs[] = {g->d_row_end, g->d_row_end32, g->d_src, g->d_weight, g->d_tile_v, g->d_head, g->d_tail, g->d_deg, g->d_val[0], g->d_val[1],
-                  g->d_cur, g->d_out_end, g->d_out_dst, g->d_out_w, g->d_fq_all, g->d_fq_new, g->d_fq_tmp, g->d_hdr_all, g->d_counters,
-                  g->d_chunk_first, g->d_chunk_vtx, g->d_partial, g->d_sync, g->d_hot_order, g->d_src_gather,
-                  g->d_carry, g->d_carry_flag, g->d_block_agg, g->d_block_flag, g->d_hot, g->d_big_list};
+  void* ptrs[] = {g->d_row_end, g->d_src, g->d_weight, g->d_deg, g->d_val[0], g->d_val[1], g->d_cur, g->d_out_end, g->d_out_dst,
+                  g->d_out_w, g->d_fq_all, g->d_fq_new, g->d_fq_tmp, g->d_hdr_all, g->d_counters, g->d_chunk_first, g->d_chunk_vtx,
+                  g->d_partial, g->d_sync, g->d_hot_order, g->d_src_gather, g->d_hot, g->d_big_list};
   for (void* p : ptrs) {
     if (!p) continue;
     if (std::find(g->host_allocs.begin(), g->host_allocs.end(), p) != g->host_allocs.end()) cudaFreeHost(p);
     else cudaFree(p);
   }
+  free_layout(g->base, /*owns_csc=*/false);
   free_layout(g->sb_main);
   free_layout(g->sb_panel);
   free_layout(g->sb_cold);
   if (g->d_cs_partial) cudaFree(g->d_cs_partial);
-  if (g->base_view.d_chain) cudaFree(g->base_view.d_chain);
   if (g->d_hub_vtx) cudaFree(g->d_hub_vtx);
   if (g->d_hub_bits) cudaFree(g->d_hub_bits);
   if (g->d_sb_partial) cudaFree(g->d_sb_partial);

@@ -8,15 +8,8 @@
 #include "seg.cuh"
 #include "push.cuh"
 
-// one CSC swept by a merge-path tile kernel, with its tile table and fix-up scratch
-struct PullLayout {
-  uint64_t* d_row_end = nullptr;    // [n_vtx + 4] (may be released once the tile table exists)
-  uint32_t* d_row_end32 = nullptr;  // [n_vtx + 8]
-  void* d_src = nullptr;            // u32 gather ids (main) or u16 block-local offsets (panel)
-  uint32_t* d_tile_v = nullptr;
-  uint32_t n_vtx = 0;
-  uint64_t e_cnt = 0;
-  uint32_t n_tiles = 0;
+// fix-up scratch of one tiled sweep (pull.cuh): per-tile partials and carries, per-block aggregates
+struct FixupScratch {
   void* d_head = nullptr;
   void* d_tail = nullptr;
   void* d_carry = nullptr;
@@ -26,6 +19,18 @@ struct PullLayout {
   uint32_t n_fix_blocks = 0;
   unsigned long long* d_chain = nullptr;  // fused fix-up: [2 * n_fix_blocks] values then [2 * n_fix_blocks] status words
   uint32_t chain_epoch = 0;
+};
+
+// one CSC swept by a merge-path tile kernel, with its tile table and fix-up scratch
+struct PullLayout {
+  uint64_t* d_row_end = nullptr;    // [n_vtx + 4] (may be released once the tile table exists)
+  uint32_t* d_row_end32 = nullptr;  // [n_vtx + 8]
+  void* d_src = nullptr;            // u32 gather ids (main) or u16 block-local offsets (panel)
+  uint32_t* d_tile_v = nullptr;
+  uint32_t n_vtx = 0;
+  uint64_t e_cnt = 0;
+  uint32_t n_tiles = 0;
+  FixupScratch fix;
   // flagged stream (seg.cuh): d_src holds the words, d_tile_v the heads before each piece, n_tiles the pieces
   uint32_t* d_close = nullptr;      // [1 + heads] vertex completed by each head
   uint32_t* d_empty = nullptr;      // vertices without edges in this stream that are not hubs
@@ -71,19 +76,12 @@ struct luxb_graph {
   uint32_t row_left = 0, n_part = 0;
   uint64_t col_left = 0, e_part = 0;
   uint64_t* d_row_end = nullptr;  // [n_part + 4] relative end offsets + sentinels
-  uint32_t* d_row_end32 = nullptr;  // [n_part + 8] low words of d_row_end (streamed by the tile kernel)
-  int pull_shape = 1;
   uint32_t* d_src = nullptr;      // [e_part + 8]
   int32_t* d_weight = nullptr;    // [e_part + 8] (col_filter)
-  uint32_t* d_tile_v = nullptr;
-  uint32_t n_tiles = 0;
-  void* d_head = nullptr;
-  void* d_tail = nullptr;
-  void* d_carry = nullptr;        // fix-up scratch (per tile / per block of tiles)
-  uint32_t* d_carry_flag = nullptr;
-  void* d_block_agg = nullptr;
-  uint32_t* d_block_flag = nullptr;
-  uint32_t n_fix_blocks = 0;
+  // the slice as swept by the merge-path kernel (pull.cuh): tile table, u32 row ends, fix-up scratch.  It borrows
+  // d_row_end from the graph and leaves d_src unset: each sweep passes the gather ids it uses.
+  PullLayout base;
+  int pull_shape = 0;             // merge-path shape (LUXB_PULL_SHAPE), chosen by finish_layout
 
   cudaStream_t stream = nullptr;
   cudaEvent_t ev_begin = nullptr, ev_end = nullptr;
@@ -155,7 +153,6 @@ struct luxb_graph {
   bool flag_barrier = true;           // LUXB_BARRIER=nccl: the 4-byte all-reduce of the communicator instead
   bool flag_barrier_all = false;      // LUXB_BARRIER=flag: also for the CC / SSSP / col_filter barriers
   bool direct_push = false;           // LUXB_PUSH=direct: owners store into EVERY rank's transfer array, no chunk pulls
-  uint64_t ag_chunk = 0, hot_chunk = 0;  // equal chunk sizes (elements) of the balanced all-gather
 
   // source-blocked PageRank sweep (panel.cuh): hub destinations x hot source blocks in shared memory
   bool empties_done[2] = {false, false};  // value buffer k already holds update(identity) at the edge-less vertices
@@ -163,9 +160,7 @@ struct luxb_graph {
   int seg_main_shape = 0, seg_panel_shape = 0;
   bool sb_on = false;
   PullLayout sb_main, sb_panel;
-  PullLayout base_view;            // the canonical CSC seen as a layout by the merge-path sweep (pull.cuh)
-  uint32_t sb_n_hub = 0, sb_n_blocks = 0, sb_bs = 0, sb_n_src = 0;
-  int sb_shape = 0;
+  uint32_t sb_n_hub = 0, sb_n_blocks = 0, sb_bs = 0;
   uint32_t* d_hub_vtx = nullptr;
   uint32_t* d_hub_bits = nullptr;
   uint32_t* d_sb_partial = nullptr;  // [NV] raw panel reductions (4-byte Acc of the app's program)
