@@ -931,12 +931,12 @@ static int reset_label_state(luxb_graph* g, bool all_active) {
 // reads, and L2 is what keeps its cold segment close.
 static constexpr double kColdSplitWindowMB = 12.0;
 static int set_l2_persisting_window(luxb_graph* g, void* base, size_t bytes) {
-  if (const char* env = getenv("LUXB_L2_PERSIST")) if (atoi(env) == 0) return 0;
+  if (!g->sweep.l2_persist) return 0;
   int max_persist = 0, max_window = 0;
   LUXB_CUDA(cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, g->cfg.device));
   LUXB_CUDA(cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, g->cfg.device));
   if (max_persist <= 0 || max_window <= 0) return 0;
-  if (const char* env = getenv("LUXB_L2_WINDOW_MB")) bytes = std::min<size_t>(bytes, (size_t)(atof(env) * 1e6));  // hottest prefix only
+  if (g->sweep.l2_window_mb >= 0) bytes = std::min<size_t>(bytes, (size_t)(g->sweep.l2_window_mb * 1e6));  // hottest prefix only
   else if (g->cs_on) bytes = std::min<size_t>(bytes, (size_t)(kColdSplitWindowMB * 1e6));
   size_t persist = std::min<size_t>((size_t)max_persist, bytes);
   LUXB_CUDA(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, persist));
@@ -953,8 +953,15 @@ static int set_l2_persisting_window(luxb_graph* g, void* base, size_t bytes) {
 
 // cold -> hub edges (PageRank, one rank) get a stream of their own when they are at least this share of the partition
 static constexpr double kColdSplitMinShare = 0.05;
-// panel tiers (build_panel_layout): a (block, hub) slot past tier 0 is kept when it expects at least this many edges
-static constexpr double kTierSlotEdges = 0.5;
+// the automatic source-blocked split, its tiers and its cold-hub stream only consider partitions of this many edges
+static constexpr uint64_t kSplitMinEdges = 1ull << 24;
+
+// May the source-blocked split (build_panel_layout) run on this partition?  It still declines after keying when the
+// panel would cover too few edges.
+static bool split_may_run(const luxb_graph* g) {
+  const SweepSettings& s = g->sweep;
+  return s.seg && s.sb != 0 && !g->cfg.zero_copy_edges && (s.sb > 0 || g->e_part >= kSplitMinEdges);
+}
 
 // Choose the hot set (largest out-degrees, at most LUXB_HOT_MB megabytes of values, default 24 MB ~ half of the H100's
 // 50 MB L2: at RMAT-27 on one H100 8 / 16 / 24 / 32 / 64 MB gave 21.4 / 15.8 / 14.2 / 16.7 / 17.3 ms per sweep) and
@@ -966,9 +973,7 @@ static int build_hot_layout(luxb_graph* g, bool compact_cold) {
   g->hot_n = 0;
   g->packed = false;
   g->cold_z = false;
-  double hot_mb = 24.0;
-  if (const char* env = getenv("LUXB_HOT_MB")) hot_mb = atof(env);
-  uint64_t h_max = (uint64_t)(hot_mb * 1e6 / 4.0);
+  uint64_t h_max = (uint64_t)(g->sweep.hot_mb * 1e6 / 4.0);
   if (h_max == 0 || g->nv < 2 || (uint64_t)g->nv >= 0xFFFFFFFFull - h_max) return 0;
   if (h_max > g->nv) h_max = g->nv;
   const int grid = g->num_sms * 8;
@@ -994,15 +999,12 @@ static int build_hot_layout(luxb_graph* g, bool compact_cold) {
   if (compact_cold && g->P == 1) {
     // one rank: the compact cold copy costs a refresh every iteration and pays for it in the cold-hub stream
     // (build_panel_layout).  LUXB_CS = 0: never, 1: always, unset: when the edges out of cold vertices are at least
-    // kColdSplitMinShare of a large partition swept by the source-blocked split (the cold-hub stream needs its hubs)
-    const char* env = getenv("LUXB_CS");
-    const int cs_mode = env ? atoi(env) : -1;
-    const char* sb = getenv("LUXB_SB");
-    const char* sweep = getenv("LUXB_SWEEP");
-    const bool no_split = (sb && atoi(sb) == 0) || (sweep && !strcmp(sweep, "merge")) || g->cfg.zero_copy_edges;
+    // kColdSplitMinShare of a large partition the source-blocked split may sweep (the cold-hub stream needs its hubs)
+    const int cs_mode = g->sweep.cs;
     uint64_t e_cold_src = 0;
     for (uint32_t d = 1; d < tau; ++d) e_cold_src += (uint64_t)d * hist[d];
-    if (cs_mode == 0 || (cs_mode < 0 && (no_split || g->e_part < (1ull << 24) || (double)e_cold_src < kColdSplitMinShare * (double)g->e_part)))
+    if (cs_mode == 0 || (cs_mode < 0 && (!split_may_run(g) || g->e_part < kSplitMinEdges ||
+                                         (double)e_cold_src < kColdSplitMinShare * (double)g->e_part)))
       compact_cold = false;
   }
   uint64_t *d_keys = nullptr, *d_keys2 = nullptr;
@@ -1100,6 +1102,7 @@ static int build_hot_layout(luxb_graph* g, bool compact_cold) {
 }
 
 static int allgather_slices(luxb_graph* g, void* replica, size_t elem_bytes);
+static void resolve_sweep_settings(SweepSettings& s);
 static int build_seg_sweep(luxb_graph* g);
 static int pagerank_publish(luxb_graph* g, float* x_new);
 static int wait_cold_exchange(luxb_graph* g);
@@ -1129,6 +1132,7 @@ int luxb_init(luxb_graph* g) {
   if (g->inited) { set_error("luxb_init called twice"); return LUXB_ERR_STATE; }
   if (g->P > 1 && !g->comm) { set_error("luxb_init: nranks > 1 needs luxb_comm_init first"); return LUXB_ERR_STATE; }
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
+  resolve_sweep_settings(g->sweep);
   const int grid = g->num_sms * 8;
   switch (g->cfg.app) {
     case LUXB_PAGERANK: {
@@ -1409,6 +1413,33 @@ static int env_int(const char* name, int dflt) {
   return e ? atoi(e) : dflt;
 }
 
+static double env_double(const char* name, double dflt) {
+  const char* e = getenv(name);
+  return e ? atof(e) : dflt;
+}
+
+// the only reader of these variables; a shape out of range falls back to shape 0
+static void resolve_sweep_settings(SweepSettings& s) {
+  s = SweepSettings();
+  if (const char* e = getenv("LUXB_SWEEP")) s.seg = strcmp(e, "merge") != 0;
+  auto shape = [](const char* name, int dflt, int n) { const int v = env_int(name, dflt); return v < 0 || v >= n ? 0 : v; };
+  s.main_shape = shape("LUXB_SEG_MAIN_SHAPE", s.main_shape, kNumSegMain);
+  s.panel_shape = shape("LUXB_SEG_PANEL_SHAPE", s.panel_shape, kNumSegPanel);
+  s.cs_shape = shape("LUXB_CS_SHAPE", s.main_shape, kNumSegMain);
+  s.sb = env_int("LUXB_SB", s.sb);
+  const int tab = kSegPanelInfo[s.panel_shape].tab;
+  s.sb_bs = std::min<uint32_t>((uint32_t)std::max(4, env_int("LUXB_SB_BS", tab)) & ~3u, (uint32_t)tab);
+  s.sb_blocks = (uint32_t)std::min(std::max(env_int("LUXB_SB_BLOCKS", (int)s.sb_blocks), 1), kPanelMaxBlocks);
+  s.sb_min_indeg = (uint32_t)std::max(env_int("LUXB_SB_MIN_INDEG", (int)s.sb_min_indeg), 1);
+  s.sb_tier = env_int("LUXB_SB_TIER", s.sb_tier);
+  s.sb_slot_edges = env_double("LUXB_SB_SLOT_EDGES", s.sb_slot_edges);
+  s.cs = env_int("LUXB_CS", s.cs);
+  s.cs_seg_mb = env_double("LUXB_CS_SEG_MB", s.cs_seg_mb);
+  s.hot_mb = env_double("LUXB_HOT_MB", s.hot_mb);
+  s.l2_persist = env_int("LUXB_L2_PERSIST", 1) != 0;
+  s.l2_window_mb = env_double("LUXB_L2_WINDOW_MB", s.l2_window_mb);
+}
+
 extern "C++" {
 // Build the flagged stream of a CSC (seg.cuh).  row_end: inclusive end offsets (u64) of n_vtx "vertices" whose edges,
 // in CSC order, carry the gather ids `ids`; blk: the vertex / edge ranges of the blocks (one block = plain stream;
@@ -1506,43 +1537,69 @@ static int build_seg_stream(luxb_graph* g, PullLayout& L, const uint64_t* d_row_
 }
 }  // extern "C++"
 
-// the whole partition as one flagged stream (PageRank without the source-blocked split)
-static int build_plain_seg_layout(luxb_graph* g) {
-  const SegShapeInfo shp = kSegMainInfo[g->seg_main_shape];
+// the main stream sb_main: every local vertex over the CSC (row_end, ids) of the edges left to it (all of them without
+// the source-blocked split; hub_bits then null)
+static int build_main_stream(luxb_graph* g, const uint64_t* d_row_end, const uint32_t* d_ids, uint64_t e_cnt, const uint32_t* hub_bits) {
+  const SegShapeInfo shp = kSegMainInfo[g->sweep.main_shape];
   StreamBlocks blk{};
   blk.n_blocks = 1;
-  blk.vfirst[0] = 0; blk.vfirst[1] = g->n_part;
-  blk.ebase[0] = 0; blk.ebase[1] = g->e_part;
-  return build_seg_stream<uint32_t, uint32_t>(g, g->sb_main, g->d_row_end, g->n_part, g->hot_n ? g->d_src_gather : g->d_src, g->e_part, blk,
-                                              (uint32_t)shp.stage_edges, (uint32_t)shp.piece, 0, true, nullptr, nullptr);
+  blk.vfirst[1] = g->n_part;
+  blk.ebase[1] = e_cnt;
+  return build_seg_stream<uint32_t, uint32_t>(g, g->sb_main, d_row_end, g->n_part, d_ids, e_cnt, blk, (uint32_t)shp.stage_edges,
+                                              (uint32_t)shp.piece, 0, true, hub_bits, nullptr);
 }
 
+extern "C++" {
+// The flagged stream of the split's groups [g0, g1) (panel.cuh): their e_cnt sorted edges (d_key / d_pay) -> ids
+// (group_fill_kernel), the CSC over their slots vbase[g0] .. vbase[g1] - 1, and the stream, whose close list holds the
+// slot numbers.  With super_end every group is padded to whole stages (the panel: a stage never straddles two source
+// blocks) and super_end receives the first stage after each; without, the groups form one block.
+template <class Word>
+static int build_group_stream(luxb_graph* g, PullLayout& L, const uint16_t* d_key, const uint64_t* d_pay, uint64_t e_cnt, uint32_t g0,
+                              uint32_t g1, const unsigned long long* hist, uint32_t bs, const SegShapeInfo& shp, uint32_t* super_end) {
+  const int grid = g->num_sms * 8;
+  const uint32_t* vbase = g->sb_groups.vbase;
+  const uint32_t v0 = vbase[g0], n_vtx = vbase[g1] - v0;
+  DevTmp tmp;
+  Word* d_ids = nullptr;
+  uint32_t* d_vcount = nullptr;
+  uint64_t* d_vrow = nullptr;
+  LUXB_TRY(tmp.alloc(&d_ids, e_cnt + 32));
+  LUXB_TRY(tmp.alloc(&d_vcount, (uint64_t)n_vtx + 1));
+  LUXB_CUDA(cudaMemsetAsync(d_vcount, 0, ((size_t)n_vtx + 1) * 4, g->stream));
+  group_fill_kernel<Word><<<grid, 256, 0, g->stream>>>(d_key, d_pay, e_cnt, g->d_src_gather, bs, g->sb_groups, v0, d_ids, d_vcount);
+  LUXB_CUDA(cudaGetLastError());
+  LUXB_TRY(tmp.alloc(&d_vrow, (uint64_t)n_vtx + 4));
+  widen_u32_to_u64_kernel<<<grid, 256, 0, g->stream>>>(d_vcount, d_vrow, n_vtx);
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceScan::InclusiveSum(t, b, d_vrow, d_vrow, (int)n_vtx, g->stream);
+  }));
+  tmp.release(d_vcount);
+  StreamBlocks blk{};
+  blk.n_blocks = super_end ? g1 - g0 : 1;
+  for (uint32_t b = 0; b < blk.n_blocks; ++b) {
+    blk.vfirst[b + 1] = super_end ? vbase[g0 + b + 1] - v0 : n_vtx;
+    blk.ebase[b + 1] = super_end ? blk.ebase[b] + hist[g0 + b] : e_cnt;
+  }
+  return build_seg_stream<Word, Word>(g, L, d_vrow, n_vtx, d_ids, e_cnt, blk, (uint32_t)shp.stage_edges, (uint32_t)shp.piece, v0, false,
+                                      nullptr, super_end);
+}
+}  // extern "C++"
+
 // Split this partition's (hot-packed) CSC into the panel (hot source block x hub destination, 15-bit offsets, gathered
-// from shared memory) and the main stream (everything else, gathered through L1).
-// LUXB_SB = 0 off / 1 force / unset: automatic (on when the panel would take at least a fifth of a large partition).
-// Tuning: LUXB_SB_BS (values per block), LUXB_SB_BLOCKS (tier 0: max blocks over all hubs), LUXB_SB_MIN_INDEG (hub
-// threshold).  Tiers (panel.cuh): the blocks after tier 0 cover the rest of the hot set, block b over the hubs of
-// in-degree d with d * m_b >= LUXB_SB_SLOT_EDGES (expected edges per slot; m_b = block b's share of the hubs' in-edges).
-// LUXB_SB_TIER = 0 off / 1 force / unset: on where the cold-hub stream may be (one rank) on a partition of >= 2^24 edges.
-// With the compact cold values of one rank (cold_z), the cold -> hub edges form a third stream (panel.cuh, ColdSplit):
-// LUXB_CS = 0 off / 1 force / unset: on when they are at least kColdSplitMinShare of the partition's edges;
-// LUXB_CS_SEG_MB: segment size (raised where the segments would not fit the sort key), LUXB_CS_SHAPE: its main shape.
+// from shared memory), with the compact cold values of one rank (cold_z) the cold-hub stream (cold source segment x hub
+// destination, panel.cuh, ColdSplit), and the main stream (everything else, gathered through L1).  Settings and their
+// automatic rules: SweepSettings.
 static int build_panel_layout(luxb_graph* g) {
   g->sb_on = false;
   g->cs_on = false;
-  const int mode = env_int("LUXB_SB", -1);
-  if (mode == 0 || g->hot_n == 0 || g->e_part == 0 || g->e_part >= 0xFFFFFFFFull || g->cfg.zero_copy_edges) return 0;
-  if (mode < 0 && g->e_part < (1ull << 24)) return 0;
-  const SegShapeInfo shp = kSegPanelInfo[g->seg_panel_shape];
-  uint32_t bs = (uint32_t)std::max(4, env_int("LUXB_SB_BS", shp.tab));
-  bs = std::min<uint32_t>(bs & ~3u, (uint32_t)shp.tab);
-  const uint32_t nb_max = (uint32_t)std::min(std::max(env_int("LUXB_SB_BLOCKS", 48), 1), kPanelMaxBlocks);
-  const uint32_t NB0 = (uint32_t)((std::min<uint64_t>(g->hot_n, (uint64_t)nb_max * bs) + bs - 1) / bs);  // tier 0
-  const int tier_mode = env_int("LUXB_SB_TIER", -1);
-  const bool tiers = tier_mode > 0 || (tier_mode < 0 && g->cold_z && g->e_part >= (1ull << 24));
+  const SweepSettings& st = g->sweep;
+  if (!split_may_run(g) || g->hot_n == 0 || g->e_part == 0 || g->e_part >= 0xFFFFFFFFull) return 0;
+  const SegShapeInfo shp = kSegPanelInfo[st.panel_shape];
+  const uint32_t bs = st.sb_bs;
+  const uint32_t NB0 = (uint32_t)((std::min<uint64_t>(g->hot_n, (uint64_t)st.sb_blocks * bs) + bs - 1) / bs);  // tier 0
+  const bool tiers = st.sb_tier > 0 || (st.sb_tier < 0 && g->cold_z && g->e_part >= kSplitMinEdges);
   const uint32_t nb_all = tiers ? (uint32_t)std::min<uint64_t>(((uint64_t)g->hot_n + bs - 1) / bs, kPanelMaxBlocks) : NB0;
-  const double slot_edges = [] { const char* e = getenv("LUXB_SB_SLOT_EDGES"); return e ? atof(e) : kTierSlotEdges; }();
-  const uint32_t min_indeg = (uint32_t)std::max(env_int("LUXB_SB_MIN_INDEG", 64), 1);
   const int grid = g->num_sms * 8;
   DevTmp tmp;
 
@@ -1550,7 +1607,7 @@ static int build_panel_layout(luxb_graph* g) {
   uint32_t *d_flag = nullptr, *d_hub_idx = nullptr;
   LUXB_TRY(tmp.alloc(&d_flag, (uint64_t)g->n_part + 1));
   LUXB_TRY(tmp.alloc(&d_hub_idx, (uint64_t)g->n_part + 1));
-  hub_flag_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, g->n_part, min_indeg, d_flag);
+  hub_flag_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, g->n_part, st.sb_min_indeg, d_flag);
   LUXB_CUDA(cudaGetLastError());
   LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
     return cub::DeviceScan::ExclusiveSum(t, b, d_flag, d_hub_idx, (int)g->n_part, g->stream);
@@ -1588,34 +1645,28 @@ static int build_panel_layout(luxb_graph* g) {
     tmp.release(d_hkey2);
     tmp.release(d_hvtx2);
   }
-  // hub prefix N_b of every block: all hubs for now (tier 0 keeps them; the tiers are decided from the first keying)
+  // hub prefix N_b of every block: all hubs in the first keying
   uint32_t NB = nb_all;
-  uint32_t n_src = (uint32_t)std::min<uint64_t>(g->hot_n, (uint64_t)NB * bs);
   std::vector<uint32_t> n_pref(NB, Nh);
   uint32_t* d_pref = nullptr;
   LUXB_TRY(tmp.alloc(&d_pref, kPanelMaxBlocks));
   LUXB_CUDA(cudaMemcpyAsync(d_pref, n_pref.data(), (size_t)NB * 4, cudaMemcpyHostToDevice, g->stream));
 
-  // cold segments: cold gather ids [H, H + C) cut into S <= 255 - NB0 segments of `seg` values, sort keys NB .. NB + S - 1
-  const int cs_mode = g->cold_z ? env_int("LUXB_CS", -1) : 0;
+  // cold segments: cold gather ids [H, H + C) cut into S <= 255 - NB0 segments of `seg` values, groups NB .. NB + S - 1
   ColdSplit cs{};
   cs.hot_n = g->hot_n;
   cs.key0 = NB;
   uint32_t S = 0;
-  if (cs_mode != 0 && g->cold_n > 0) {
-    const char* env = getenv("LUXB_CS_SEG_MB");
-    const double seg_mb = env ? atof(env) : 24.0;
+  if (g->cold_z && st.cs != 0 && g->cold_n > 0) {
     const uint32_t s_max = 255 - NB0;
-    uint64_t seg = std::max<uint64_t>(1, (uint64_t)(seg_mb * 1e6 / 4.0));
+    uint64_t seg = std::max<uint64_t>(1, (uint64_t)(st.cs_seg_mb * 1e6 / 4.0));
     seg = std::min<uint64_t>(std::max<uint64_t>(seg, (g->cold_n + s_max - 1) / s_max), g->cold_n);
-    S = (uint32_t)((g->cold_n + seg - 1) / seg);
-    if ((uint64_t)Nh * S < 0x7FFFFFF0ull) cs.seg = (uint32_t)seg;
+    const uint32_t n_seg = (uint32_t)((g->cold_n + seg - 1) / seg);
+    if ((uint64_t)Nh * n_seg < 0x7FFFFFF0ull) { cs.seg = (uint32_t)seg; S = n_seg; }
   }
-  uint32_t* d_cold_cnt = nullptr;
-  if (cs.seg) LUXB_TRY(tmp.alloc(&d_cold_cnt, Nh));
 
-  // 2. edge keys: block of the source for (hot source, hub destination in the block's prefix) edges, cold segment + NB
-  // for (cold source, hub destination) edges if the cold split is on, kSplitKeyMain for the rest; 3. stable sort
+  // 2. edge keys: the group of the edge for (hot source, hub destination in the block's prefix) and (cold source, hub
+  // destination) edges, kSplitKeyMain for the rest; then the key histogram
   uint16_t *d_key = nullptr, *d_key2 = nullptr;
   uint64_t *d_pay = nullptr, *d_pay2 = nullptr;
   LUXB_TRY(tmp.alloc(&d_key, g->e_part));
@@ -1626,45 +1677,50 @@ static int build_panel_layout(luxb_graph* g) {
   unsigned long long* d_hist = nullptr;
   LUXB_TRY(tmp.alloc(&d_hist, kBins));
   unsigned long long hist[kBins];
-  bool tiers_open = tiers && NB > NB0;  // the tier prefixes still have to be chosen from this keying's histogram
-  for (;;) {
+  auto key_edges = [&]() -> int {
+    const uint32_t n_src = (uint32_t)std::min<uint64_t>(g->hot_n, (uint64_t)NB * bs);
     edge_iota_kernel<<<grid, 256, 0, g->stream>>>(d_pay, d_key, g->e_part);
-    hub_key_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, g->d_src_gather, d_hub_vtx, Nh, n_src, bs, d_pref, NB, d_key, d_pay, d_cov,
-                                                cs, d_cold_cnt);
+    hub_key_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, g->d_src_gather, d_hub_vtx, Nh, n_src, bs, d_pref, NB, d_key, d_pay, d_cov, cs);
     LUXB_CUDA(cudaMemsetAsync(d_hist, 0, kBins * 8, g->stream));
     key_hist_kernel<<<grid, 256, 0, g->stream>>>(d_key, g->e_part, d_hist);
     LUXB_CUDA(cudaGetLastError());
     LUXB_CUDA(cudaMemcpyAsync(hist, d_hist, sizeof(hist), cudaMemcpyDeviceToHost, g->stream));
     LUXB_CUDA(cudaStreamSynchronize(g->stream));
-    if (tiers_open) {
-      // block b >= NB0 keeps hub h while d_h * m_b >= slot_edges, m_b = (edges block b -> hubs) / (edges into hubs)
-      tiers_open = false;
-      uint64_t e_hub = 0;
-      for (uint32_t h = 0; h < Nh; ++h) e_hub += ~hub_key[h];
-      for (uint32_t b = NB0; b < NB; ++b) {
-        uint32_t keep = 0;
-        if (hist[b] > 0) {
-          const double d_min = slot_edges * (double)e_hub / (double)hist[b];
-          // hub_key ascends (~in-degree): the hubs with in-degree >= d_min are a prefix
-          keep = (uint32_t)(std::partition_point(hub_key.begin(), hub_key.end(), [&](uint32_t k) { return (double)~k >= d_min; }) - hub_key.begin());
-        }
-        n_pref[b] = std::min(keep, n_pref[b - 1]);
+    return 0;
+  };
+  LUXB_TRY(key_edges());
+  // Both decisions come from this first histogram.  Tiers: block b >= NB0 keeps hub h while d_h * m_b >= slot_edges,
+  // m_b = (edges block b -> hubs) / (edges into hubs).  Cold-hub verdict: a cold key only needs a cold source (never
+  // below n_src) and a hub destination, so fewer blocks renumber the segments without moving an edge.
+  bool rekey = false;
+  if (tiers && NB > NB0) {
+    uint64_t e_hub = 0;
+    for (uint32_t h = 0; h < Nh; ++h) e_hub += ~hub_key[h];
+    for (uint32_t b = NB0; b < NB; ++b) {
+      uint32_t keep = 0;
+      if (hist[b] > 0) {
+        const double d_min = st.sb_slot_edges * (double)e_hub / (double)hist[b];
+        // hub_key ascends (~in-degree): the hubs with in-degree >= d_min are a prefix
+        keep = (uint32_t)(std::partition_point(hub_key.begin(), hub_key.end(), [&](uint32_t k) { return (double)~k >= d_min; }) - hub_key.begin());
       }
-      while (NB > NB0 && n_pref[NB - 1] == 0) --NB;
-      n_src = (uint32_t)std::min<uint64_t>(g->hot_n, (uint64_t)NB * bs);
-      cs.key0 = NB;
-      LUXB_CUDA(cudaMemcpyAsync(d_pref, n_pref.data(), (size_t)NB * 4, cudaMemcpyHostToDevice, g->stream));
-      continue;
+      n_pref[b] = std::min(keep, n_pref[b - 1]);
+      rekey |= n_pref[b] < Nh;
     }
-    uint64_t e_cs = 0;
-    for (uint32_t s = 0; s < S; ++s) e_cs += hist[NB + s];
-    if (cs.seg == 0 || cs_mode > 0 || (e_cs > 0 && (double)e_cs >= kColdSplitMinShare * (double)g->e_part)) break;
-    cs.seg = 0;  // automatic and too few cold -> hub edges: key again without the cold split
+    while (NB > NB0 && n_pref[NB - 1] == 0) --NB;
+    cs.key0 = NB;
+    LUXB_CUDA(cudaMemcpyAsync(d_pref, n_pref.data(), (size_t)NB * 4, cudaMemcpyHostToDevice, g->stream));
   }
-  if (cs.seg == 0) S = 0;
+  uint64_t e_cs = 0;
+  for (uint32_t s = 0; s < S; ++s) e_cs += hist[nb_all + s];
+  if (S && st.cs < 0 && !(e_cs > 0 && (double)e_cs >= kColdSplitMinShare * (double)g->e_part)) {
+    rekey |= e_cs > 0;  // automatic and too few cold -> hub edges: no cold split
+    cs.seg = 0;
+    S = 0;
+  }
+  if (rekey) LUXB_TRY(key_edges());
   {
-    // two stable sorts: by hub position (payload bits 32.., 0 for main edges), then by key.  Every block and segment
-    // then lists its edges by virtual vertex (hub order is not id order), the main stream keeps the CSC order.
+    // 3. two stable sorts: by hub position (payload bits 32.., 0 for main edges), then by key.  Every group then lists
+    // its edges by slot (hub order is not id order), the main stream keeps the CSC order.
     cub::DoubleBuffer<uint16_t> kb(d_key, d_key2);
     cub::DoubleBuffer<uint64_t> pb(d_pay, d_pay2);
     int hbits = 1;
@@ -1690,81 +1746,32 @@ static int build_panel_layout(luxb_graph* g) {
               (unsigned long long)e_main, (unsigned long long)g->e_part);
     return LUXB_ERR_STATE;
   }
-  if (e_cov == 0 || (mode < 0 && e_cov < g->e_part / 5)) return 0;
+  if (e_cov == 0 || (st.sb < 0 && e_cov < g->e_part / 5)) return 0;
 
-  // 4. panel CSC over virtual vertices (block b, hub h < N_b) -> index vbase[b] + h: offsets + per-vertex in-degree
-  uint64_t nv_total = 0;
-  for (uint32_t b = 0; b < NB; ++b) nv_total += n_pref[b];
-  LUXB_ARG(nv_total < 0x7FFFFFF0ull, "panel: too many (block, hub) slots");
-  const uint32_t NV = (uint32_t)nv_total;
-  StreamBlocks pblk{};
-  pblk.n_blocks = NB;
-  g->sb_pb = PanelBases{};
-  for (uint32_t b = 0; b <= NB; ++b) {
-    g->sb_pb.vbase[b] = b == 0 ? 0 : g->sb_pb.vbase[b - 1] + n_pref[b - 1];
-    pblk.vfirst[b] = g->sb_pb.vbase[b];
+  // 4. the group table: block b serves N_b hubs, a cold segment all Nh; slot vbase[g] + h
+  const uint32_t NG = NB + S;
+  LUXB_ARG(NG < kSplitKeyMain, "panel: too many source groups");
+  uint64_t n_slots = 0;
+  g->sb_groups = SplitGroups{};
+  for (uint32_t k = 0; k < NG; ++k) {
+    n_slots += k < NB ? n_pref[k] : Nh;
+    LUXB_ARG(n_slots < 0x7FFFFFF0ull, "panel: too many (group, hub) slots");
+    g->sb_groups.vbase[k + 1] = (uint32_t)n_slots;
   }
-  pblk.ebase[0] = 0;
-  for (uint32_t b = 0; b < NB; ++b) pblk.ebase[b + 1] = pblk.ebase[b] + hist[b];
-  uint16_t* d_src16 = nullptr;
-  uint32_t* d_vcount = nullptr;
-  uint64_t* d_vrow = nullptr;
-  LUXB_TRY(tmp.alloc(&d_src16, e_cov + 32));
-  LUXB_TRY(tmp.alloc(&d_vcount, (uint64_t)NV + 1));
-  LUXB_CUDA(cudaMemsetAsync(d_vcount, 0, ((size_t)NV + 1) * 4, g->stream));
-  panel_fill_kernel<<<grid, 256, 0, g->stream>>>(d_key2, d_pay2, e_cov, g->d_src_gather, bs, g->sb_pb, d_src16, d_vcount);
-  LUXB_CUDA(cudaGetLastError());
-  LUXB_TRY(tmp.alloc(&d_vrow, (uint64_t)NV + 4));
-  widen_u32_to_u64_kernel<<<grid, 256, 0, g->stream>>>(d_vcount, d_vrow, NV);
-  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
-    return cub::DeviceScan::InclusiveSum(t, b, d_vrow, d_vrow, (int)NV, g->stream);
-  }));
-  tmp.release(d_vcount);
-  LUXB_TRY((build_seg_stream<uint16_t, uint16_t>(g, g->sb_panel, d_vrow, NV, d_src16, e_cov, pblk, (uint32_t)shp.stage_edges,
-                                                 (uint32_t)shp.piece, 0, false, nullptr, g->sb_super_end)));
-  tmp.release(d_vrow);
-  tmp.release(d_src16);
+  // 5. the panel (per-block stage padding) and the cold-hub stream (one block: its kernel claims stages in order, so the
+  // SMs move through the segments together)
+  LUXB_TRY(build_group_stream<uint16_t>(g, g->sb_panel, d_key2, d_pay2, e_cov, 0, NB, hist, bs, shp, g->sb_super_end));
+  if (S)
+    LUXB_TRY(build_group_stream<uint32_t>(g, g->sb_cold, d_key2 + e_cov, d_pay2 + e_cov, e_cold, NB, NG, hist, 0,
+                                          kSegMainInfo[st.cs_shape], nullptr));
 
-  // 4b. cold-hub CSC over virtual vertices (segment s, hub h) -> index s * Nh + h, gather ids unchanged: one block,
-  // no padding between segments (its kernel claims stages in order, so the SMs move through the segments together)
-  if (S) {
-    const uint32_t NVc = Nh * S;
-    uint32_t *d_cids = nullptr, *d_ccount = nullptr;
-    uint64_t* d_crow = nullptr;
-    LUXB_TRY(tmp.alloc(&d_cids, e_cold + 8));
-    LUXB_TRY(tmp.alloc(&d_ccount, (uint64_t)NVc + 1));
-    LUXB_CUDA(cudaMemsetAsync(d_ccount, 0, ((size_t)NVc + 1) * 4, g->stream));
-    cold_fill_kernel<<<grid, 256, 0, g->stream>>>(d_key2 + e_cov, d_pay2 + e_cov, e_cold, g->d_src_gather, NB, Nh, d_cids, d_ccount);
-    LUXB_CUDA(cudaGetLastError());
-    LUXB_TRY(tmp.alloc(&d_crow, (uint64_t)NVc + 4));
-    widen_u32_to_u64_kernel<<<grid, 256, 0, g->stream>>>(d_ccount, d_crow, NVc);
-    LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
-      return cub::DeviceScan::InclusiveSum(t, b, d_crow, d_crow, (int)NVc, g->stream);
-    }));
-    tmp.release(d_ccount);
-    g->cs_shape = env_int("LUXB_CS_SHAPE", g->seg_main_shape);
-    if (g->cs_shape < 0 || g->cs_shape >= kNumSegMain) g->cs_shape = 0;
-    const SegShapeInfo cshp = kSegMainInfo[g->cs_shape];
-    StreamBlocks cblk{};
-    cblk.n_blocks = 1;
-    cblk.vfirst[0] = 0; cblk.vfirst[1] = NVc;
-    cblk.ebase[0] = 0; cblk.ebase[1] = e_cold;
-    LUXB_TRY((build_seg_stream<uint32_t, uint32_t>(g, g->sb_cold, d_crow, NVc, d_cids, e_cold, cblk, (uint32_t)cshp.stage_edges,
-                                                   (uint32_t)cshp.piece, 0, false, nullptr, nullptr)));
-    tmp.release(d_crow);
-    tmp.release(d_cids);
-    // raw cold-hub sums: (segment, hub) pairs without edges keep the identity (0: PageRank only)
-    LUXB_TRY(dmalloc(&g->d_cs_partial, (uint64_t)NVc + 1));
-    LUXB_CUDA(cudaMemsetAsync(g->d_cs_partial, 0, ((size_t)NVc + 1) * 4, g->stream));
-  }
-
-  // 5. main stream: what is left, in the original (dst, src) order
+  // 6. main stream: what is left, in the original (dst, src) order
   uint32_t* d_main_src = nullptr;
   uint64_t* d_main_row = nullptr;
   LUXB_TRY(tmp.alloc(&d_main_src, e_main + 8));
   main_fill_kernel<<<grid, 256, 0, g->stream>>>(d_pay2 + e_cov + e_cold, e_main, g->d_src_gather, d_main_src);
   LUXB_TRY(tmp.alloc(&d_main_row, (uint64_t)g->n_part + 4));
-  main_indeg_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, g->n_part, d_flag, d_hub_idx, d_cov, S ? d_cold_cnt : nullptr, d_main_row);
+  main_indeg_kernel<<<grid, 256, 0, g->stream>>>(g->d_row_end, g->n_part, d_flag, d_hub_idx, d_cov, d_main_row);
   LUXB_CUDA(cudaGetLastError());
   LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
     return cub::DeviceScan::InclusiveSum(t, b, d_main_row, d_main_row, (int)g->n_part, g->stream);
@@ -1775,30 +1782,24 @@ static int build_panel_layout(luxb_graph* g) {
   if (chk != e_main) { set_error("panel split: offsets do not add up"); return LUXB_ERR_STATE; }
   tmp.release(d_key2);
   tmp.release(d_pay2);
-  const SegShapeInfo mshp = kSegMainInfo[g->seg_main_shape];
-  StreamBlocks mblk{};
-  mblk.n_blocks = 1;
-  mblk.vfirst[0] = 0; mblk.vfirst[1] = g->n_part;
-  mblk.ebase[0] = 0; mblk.ebase[1] = e_main;
-  LUXB_TRY((build_seg_stream<uint32_t, uint32_t>(g, g->sb_main, d_main_row, g->n_part, d_main_src, e_main, mblk, (uint32_t)mshp.stage_edges,
-                                                 (uint32_t)mshp.piece, 0, true, d_hub_bits, nullptr)));
+  LUXB_TRY(build_main_stream(g, d_main_row, d_main_src, e_main, d_hub_bits));
   tmp.release(d_main_row);
   tmp.release(d_main_src);
 
-  // 6. raw panel sums: one slot per (block, hub); slots of (block, hub) pairs without edges stay 0 forever
-  // (the program's identity: 0 bits for sums and max labels, all ones for min distances)
-  LUXB_TRY(dmalloc(&g->d_sb_partial, (uint64_t)NV + 1));
-  LUXB_CUDA(cudaMemsetAsync(g->d_sb_partial, g->cfg.app == LUXB_SSSP ? 0xFF : 0, ((size_t)NV + 1) * 4, g->stream));
+  // 7. raw sums of every (group, hub) slot; slots without edges keep the program's identity forever (0 bits for sums
+  // and max labels, all ones for min distances; the cold-hub stream is PageRank only)
+  LUXB_TRY(dmalloc(&g->d_sb_partial, (uint64_t)n_slots + 1));
+  LUXB_CUDA(cudaMemsetAsync(g->d_sb_partial, g->cfg.app == LUXB_SSSP ? 0xFF : 0, ((size_t)n_slots + 1) * 4, g->stream));
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
   g->d_hub_vtx = d_hub_vtx; tmp.keep(d_hub_vtx);
   g->d_hub_bits = d_hub_bits; tmp.keep(d_hub_bits);
   g->sb_n_hub = Nh;
   g->sb_n_blocks = NB;
+  g->sb_n_groups = NG;
   g->sb_bs = bs;
   g->sb_on = true;
   g->cs_on = S > 0;
-  g->cs_n_seg = S;
-  g->cs_seg = cs.seg;
+  const uint64_t NV = g->sb_groups.vbase[NB];
   g->stats.panel_edges = e_cov0;
   g->stats.panel_hubs = Nh;
   g->stats.panel_blocks = NB0;
@@ -1810,7 +1811,7 @@ static int build_panel_layout(luxb_graph* g) {
   if (g->cfg.verbose)
     printf("[luxb rank %d] source-blocked sweep: %u hub destinations (in-degree >= %u) x %u blocks of %u hot sources, + %u tier blocks "
            "(%llu slots, %llu edges); panel %llu edges (%.1f %%), cold-hub %llu edges (%u segments of %u values), main %llu edges\n",
-           g->cfg.rank, Nh, min_indeg, NB0, bs, NB - NB0, (unsigned long long)(NV - (uint64_t)NB0 * Nh), (unsigned long long)(e_cov - e_cov0),
+           g->cfg.rank, Nh, st.sb_min_indeg, NB0, bs, NB - NB0, (unsigned long long)(NV - (uint64_t)NB0 * Nh), (unsigned long long)(e_cov - e_cov0),
            (unsigned long long)e_cov, 100.0 * e_cov / g->e_part, (unsigned long long)e_cold, S, cs.seg, (unsigned long long)e_main);
   return 0;
 }
@@ -1820,18 +1821,10 @@ static int build_panel_layout(luxb_graph* g) {
 static int build_seg_sweep(luxb_graph* g) {
   g->seg_on = false;
   g->sb_on = false;
-  if (const char* env = getenv("LUXB_SWEEP")) if (!strcmp(env, "merge")) return 0;
+  if (!g->sweep.seg) return 0;
   if (g->n_part == 0 || g->cfg.zero_copy_edges || g->e_part >= 0xFFFFFFF0ull) return 0;  // zero-copy graphs keep the canonical arrays
-  g->seg_main_shape = env_int("LUXB_SEG_MAIN_SHAPE", 6);
-  if (g->seg_main_shape < 0 || g->seg_main_shape >= kNumSegMain) g->seg_main_shape = 0;
-  g->seg_panel_shape = env_int("LUXB_SEG_PANEL_SHAPE", 1);
-  if (g->seg_panel_shape < 0 || g->seg_panel_shape >= kNumSegPanel) g->seg_panel_shape = 0;
   LUXB_TRY(build_panel_layout(g));
-  if (!g->cs_on) free_layout(g->sb_cold);
-  if (!g->sb_on) {
-    free_layout(g->sb_panel);
-    LUXB_TRY(build_plain_seg_layout(g));
-  }
+  if (!g->sb_on) LUXB_TRY(build_main_stream(g, g->d_row_end, g->hot_n ? g->d_src_gather : g->d_src, g->e_part, nullptr));
   g->seg_on = true;
   return 0;
 }
@@ -1907,7 +1900,7 @@ static int launch_seg_main(luxb_graph* g, PullLayout& L, const typename Prog::Ve
   a.p.hub_bits = hub_bits;
   a.p.l2_hints = g->l2_hints;
   LUXB_TRY(wait_cold_exchange(g));
-  LUXB_TRY((launch_seg_stream<false, Prog>(g, L, a, g->seg_main_shape, g->pull_ctas, 2, 0, "seg")));
+  LUXB_TRY((launch_seg_stream<false, Prog>(g, L, a, g->sweep.main_shape, g->pull_ctas, 2, 0, "seg")));
   // vertices without in-edges in this stream.  PageRank: update(identity) is a constant -> written once per value
   // buffer.  Hubs among them need the raw identity every sweep (the combine overwrites it).
   if (out_buffer >= 0 && L.n_empty && !g->empties_done[out_buffer]) {
@@ -1939,21 +1932,21 @@ static int sweep_seg(luxb_graph* g, const typename Prog::Vertex* x_nat, const ty
     pa.bs = g->sb_bs;
     pa.n_blocks = g->sb_n_blocks;
     for (uint32_t b = 0; b < g->sb_n_blocks; ++b) pa.super_end[b] = g->sb_super_end[b];
-    LUXB_TRY((launch_seg_stream<true, Prog>(g, g->sb_panel, pa, g->seg_panel_shape, 1, 4, 5, "panel")));
+    LUXB_TRY((launch_seg_stream<true, Prog>(g, g->sb_panel, pa, g->sweep.panel_shape, 1, 4, 5, "panel")));
     pt_mark(g, 1);
   }
   if (g->cs_on) {
-    // cold-hub stream: raw partial per (cold segment, hub); its gathers all index the compact cold values, which it
+    // cold-hub stream: raw partial per (cold segment, hub) slot; its gathers all index the compact cold values, which it
     // loads with evict_normal (l2_hints = 0): the current segment is meant to stay in L2 while the SMs sweep it
     SegArgs<Prog> ca{};
     ca.p.x_old = x_cold;
     ca.p.x_hot = reinterpret_cast<const typename Prog::Vertex*>(g->d_hot);
     ca.p.hot_n = g->hot_n;
-    ca.p.out = reinterpret_cast<typename Prog::Vertex*>(g->d_cs_partial);
+    ca.p.out = reinterpret_cast<typename Prog::Vertex*>(g->d_sb_partial);
     ca.p.raw_out = 1;
     ca.p.l2_hints = 0;
     ca.p.prm = prm;
-    LUXB_TRY((launch_seg_stream<false, Prog>(g, g->sb_cold, ca, g->cs_shape, g->pull_ctas, 4, 9, "cold-hub")));
+    LUXB_TRY((launch_seg_stream<false, Prog>(g, g->sb_cold, ca, g->sweep.cs_shape, g->pull_ctas, 4, 9, "cold-hub")));
     pt_mark(g, 1);
   }
   LUXB_TRY((launch_seg_main<Prog>(g, g->sb_main, x_nat, x_cold, out_local, out_buffer, prm, g->sb_on ? g->d_hub_bits : nullptr)));
@@ -1963,11 +1956,10 @@ static int sweep_seg(luxb_graph* g, const typename Prog::Vertex* x_nat, const ty
     ca.hub_vtx = g->d_hub_vtx;
     ca.n_hub = g->sb_n_hub;
     ca.n_blocks = g->sb_n_blocks;
+    ca.n_groups = g->sb_n_groups;
     ca.row_left = g->row_left;
-    ca.pb = g->sb_pb;
+    ca.sg = g->sb_groups;
     ca.partial = reinterpret_cast<const Acc*>(g->d_sb_partial);
-    ca.cold_partial = reinterpret_cast<const Acc*>(g->d_cs_partial);
-    ca.n_cold_seg = g->cs_on ? g->cs_n_seg : 0;
     ca.x_nat = x_nat;
     ca.out = out_local;
     ca.prm = prm;
@@ -2691,7 +2683,6 @@ void luxb_close(luxb_graph* g) {
   free_layout(g->sb_main);
   free_layout(g->sb_panel);
   free_layout(g->sb_cold);
-  if (g->d_cs_partial) cudaFree(g->d_cs_partial);
   if (g->d_hub_vtx) cudaFree(g->d_hub_vtx);
   if (g->d_hub_bits) cudaFree(g->d_hub_bits);
   if (g->d_sb_partial) cudaFree(g->d_sb_partial);

@@ -41,6 +41,27 @@ struct PullLayout {
   uint64_t n_words = 0;
 };
 
+// How the gather side and the pull sweeps are laid out (api.cu: build_hot_layout, build_panel_layout), read from the
+// environment once at luxb_init (resolve_sweep_settings).  Modes: -1 (unset) automatic, 0 off, 1 forced.
+struct SweepSettings {
+  bool seg = true;             // LUXB_SWEEP=merge: the merge-path tiles of pull.cuh instead of the flagged streams
+  int main_shape = 6, panel_shape = 1, cs_shape = 6;  // LUXB_SEG_MAIN_SHAPE, LUXB_SEG_PANEL_SHAPE, LUXB_CS_SHAPE (= main)
+  int sb = -1;                 // LUXB_SB: the source-blocked split, automatic when the panel takes >= 1/5 of a large partition
+  uint32_t sb_bs = 0;          // LUXB_SB_BS: values per hot source block (a multiple of 4, <= the panel table)
+  uint32_t sb_blocks = 48;     // LUXB_SB_BLOCKS: tier 0, at most this many blocks over all hubs
+  uint32_t sb_min_indeg = 64;  // LUXB_SB_MIN_INDEG: hub threshold
+  // LUXB_SB_TIER: blocks past tier 0 over the rest of the hot set (automatic: where the cold-hub stream may be, on a
+  // large partition), block b over the hubs of in-degree d with d * m_b >= LUXB_SB_SLOT_EDGES (expected edges per
+  // slot; m_b = block b's share of the hubs' in-edges)
+  int sb_tier = -1;
+  double sb_slot_edges = 0.5;
+  int cs = -1;                 // LUXB_CS: the cold-hub stream, automatic when its edges are >= kColdSplitMinShare
+  double cs_seg_mb = 24.0;     // LUXB_CS_SEG_MB: its source segment (raised where the segments would not fit the keys)
+  double hot_mb = 24.0;        // LUXB_HOT_MB: the hot set
+  bool l2_persist = true;      // LUXB_L2_PERSIST=0: no persisting L2 window
+  double l2_window_mb = -1.0;  // LUXB_L2_WINDOW_MB: cap on that window (< 0: unset)
+};
+
 // dev aid: LUXB_PHASE_TIMING=1 prints the mean device time of each phase of a PageRank iteration at luxb_close
 struct PhaseTimer {
   bool on = false, per_call = false;
@@ -154,26 +175,24 @@ struct luxb_graph {
   bool flag_barrier_all = false;      // LUXB_BARRIER=flag: also for the CC / SSSP / col_filter barriers
   bool direct_push = false;           // LUXB_PUSH=direct: owners store into EVERY rank's transfer array, no chunk pulls
 
+  SweepSettings sweep;
+
   // source-blocked PageRank sweep (panel.cuh): hub destinations x hot source blocks in shared memory
   bool empties_done[2] = {false, false};  // value buffer k already holds update(identity) at the edge-less vertices
   bool seg_on = false;             // PageRank sweeps the flagged stream(s) of seg.cuh (sb_main [+ sb_panel])
-  int seg_main_shape = 0, seg_panel_shape = 0;
   bool sb_on = false;
   PullLayout sb_main, sb_panel;
-  uint32_t sb_n_hub = 0, sb_n_blocks = 0, sb_bs = 0;
+  uint32_t sb_n_hub = 0, sb_n_blocks = 0, sb_n_groups = 0, sb_bs = 0;  // groups: sb_n_blocks panel blocks, then cold segments
   uint32_t* d_hub_vtx = nullptr;
   uint32_t* d_hub_bits = nullptr;
-  uint32_t* d_sb_partial = nullptr;  // [NV] raw panel reductions (4-byte Acc of the app's program)
-  luxb::PanelBases sb_pb{};
+  uint32_t* d_sb_partial = nullptr;  // [vbase[sb_n_groups]] raw reductions of every (group, hub) slot (4-byte Acc)
+  luxb::SplitGroups sb_groups{};
   uint32_t sb_super_end[luxb::kPanelMaxBlocks]{};
   // cold-hub stream (PageRank, one rank): cold source segment x hub destination, gathered through L1 from an L2-sized
   // segment of the compact cold values (panel.cuh, ColdSplit)
   bool cold_z = false;             // one rank: d_hot = Z = [hot copies | cold-active values in id order], d_hot_order covers both
   bool cs_on = false;
-  int cs_shape = 0;                // main shape of the cold-hub stream's kernel (LUXB_CS_SHAPE)
   PullLayout sb_cold;
-  uint32_t cs_n_seg = 0, cs_seg = 0;
-  uint32_t* d_cs_partial = nullptr;  // [cs_n_seg * sb_n_hub] raw cold-hub reductions
 
   // launch configuration resolved once at open time (no getenv / function-static state on the hot path)
   int pull_ctas = 3;

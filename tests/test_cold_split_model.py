@@ -3,12 +3,15 @@ build_hot_layout / build_panel_layout, panel.cuh), checked against per-vertex su
 
   * gather space Z = [hot copies | cold-active values (0 < out-degree < tau) in id order]; a source's gather id is its
     hot rank or H + its cold rank, and one gather over [hot order | cold list] refreshes all of Z    (build_hot_layout)
-  * edge keys: (hot source of block b -> hub) = b, (cold source of segment s -> hub) = NB + s, the rest 255; segments
-    of `seg` values, raised so that NB + S <= 255; one stable sort separates panel, cold-hub and main   (hub_key_kernel)
-  * panel and cold-hub streams over virtual vertices b * Nh + h and s * Nh + h; main in-degree = in-degree minus both
-    coverage counts                                        (panel_fill_kernel, cold_fill_kernel, main_indeg_kernel)
+  * edge keys = source groups: (hot source of block b -> hub) = b, (cold source of segment s -> hub) = NB + s, the
+    rest 511 (kSplitKeyMain); segments of `seg` values, raised so that S <= 255 - NB; one stable sort separates panel,
+    cold-hub and main                                                                             (hub_key_kernel)
+  * one table of groups: group g (block b = g, or segment s = g - NB) serves every hub here (no tiers) and owns the
+    slots vbase[g] + h of one raw-partial array; the panel stream covers the slots of groups [0, NB), the cold-hub
+    stream those of [NB, NB + S), its close list carrying slot numbers; main in-degree = in-degree minus the edges
+    of both                                                              (group_fill_kernel, main_indeg_kernel)
   * each stream swept by the flagged-stream model of test_seg_model.py; hubs = main raw sum + panel partials in block
-    order + cold partials in segment order                                                      (combine_hub_kernel)
+    order + cold partials in segment order, all read from that array                            (combine_hub_kernel)
 Integer edge values make every summation order exact, so the comparison is bit-exact."""
 import numpy as np
 import pytest
@@ -18,6 +21,7 @@ from graphs import in_degrees, rmat
 from test_seg_model import direct_sums, run_model
 
 CAP = 4096
+KEY_MAIN = 511  # kSplitKeyMain
 
 
 def hot_cold_layout(row_end, src, hot_mb):
@@ -44,7 +48,8 @@ def hot_cold_layout(row_end, src, hot_mb):
 
 
 def split(row_end, gid, H, n_cold, min_indeg, bs, nb_max, seg_values):
-    """Keys of every edge, block / segment counts and the three CSCs as {stream: (row_end, edge indices)}."""
+    """Keys of every edge, block / segment counts, the group table and the three CSCs as
+    {stream: (row_end, edge indices, first slot)}."""
     nv = len(row_end)
     indeg = in_degrees(row_end)
     dst = np.repeat(np.arange(nv), indeg)
@@ -56,37 +61,40 @@ def split(row_end, gid, H, n_cold, min_indeg, bs, nb_max, seg_values):
     s_max = 255 - NB
     seg = min(max(seg_values, -(-n_cold // s_max)), n_cold)
     S = -(-n_cold // seg)
-    key = np.full(len(gid), 255, np.int64)
+    key = np.full(len(gid), KEY_MAIN, np.int64)
     hub_e = is_hub[dst]
     key[hub_e & (gid < n_src)] = gid[hub_e & (gid < n_src)] // bs
     c = hub_e & (gid >= H)
     key[c] = NB + (gid[c] - H) // seg
-    assert key[key != 255].max(initial=0) < 255
+    assert key[key != KEY_MAIN].max(initial=0) < KEY_MAIN
     order = np.argsort(key, kind="stable")
     k_sorted = key[order]
+    vbase = np.arange(NB + S + 1, dtype=np.int64) * Nh  # every group serves all Nh hubs
     streams = {}
-    for name, lo, hi, n_virt, vid in (("panel", 0, NB, NB * Nh, lambda e, k: k * Nh + hub_idx[dst[e]]),
-                                      ("cold", NB, NB + S, S * Nh, lambda e, k: (k - NB) * Nh + hub_idx[dst[e]])):
+    for name, lo, hi in (("panel", 0, NB), ("cold", NB, NB + S)):
         sel = order[(k_sorted >= lo) & (k_sorted < hi)]
-        v = vid(sel, key[sel])
-        assert np.all(np.diff(v) >= 0)  # the stable sort leaves every virtual vertex's edges contiguous, in order
-        streams[name] = (np.cumsum(np.bincount(v, minlength=n_virt)).astype(np.uint64), sel)
-    main = order[k_sorted == 255]
-    cov = np.bincount(dst[order[k_sorted != 255]], minlength=nv)
-    streams["main"] = (np.cumsum(indeg - cov).astype(np.uint64), main)
-    return streams, NB, S, seg, Nh, is_hub
+        v = vbase[key[sel]] + hub_idx[dst[sel]]
+        assert np.all(np.diff(v) >= 0)  # the stable sort leaves every slot's edges contiguous, in order
+        v0 = int(vbase[lo])
+        streams[name] = (np.cumsum(np.bincount(v - v0, minlength=int(vbase[hi]) - v0)).astype(np.uint64), sel, v0)
+    main = order[k_sorted == KEY_MAIN]
+    cov = np.bincount(dst[order[k_sorted != KEY_MAIN]], minlength=nv)
+    streams["main"] = (np.cumsum(indeg - cov).astype(np.uint64), main, 0)
+    return streams, NB, S, seg, vbase, is_hub
 
 
-def sweep_and_combine(streams, vals, NB, S, Nh, is_hub, drop_last_segment=False):
+def sweep_and_combine(streams, vals, NB, S, vbase, is_hub, drop_last_segment=False):
     shape = dict(piece=16, rnd=8, stage=32)
-    raw = {name: run_model(re, vals[sel], **shape) for name, (re, sel) in streams.items()}
+    raw = {name: {v0 + v: x for v, x in run_model(re, vals[sel], **shape).items()} for name, (re, sel, v0) in streams.items()}
+    assert not raw["panel"].keys() & raw["cold"].keys()
+    partial = {**raw["panel"], **raw["cold"]}  # one array of (group, hub) slots
     out = dict(raw["main"])
     for h, v in enumerate(np.nonzero(is_hub)[0]):
         t = raw["main"].get(int(v), 0)
         for b in range(NB):
-            t += raw["panel"].get(b * Nh + h, 0)
-        for s in range(S - (1 if drop_last_segment else 0)):
-            t += raw["cold"].get(s * Nh + h, 0)
+            t += partial.get(int(vbase[b]) + h, 0)
+        for g in range(NB, NB + S - (1 if drop_last_segment else 0)):
+            t += partial.get(int(vbase[g]) + h, 0)
         out[int(v)] = t
     return out
 
@@ -107,13 +115,14 @@ def test_three_way_split(case):
     row_end, src = rmat(int(name[len("rmat"):]))
     H, gid, zsrc = hot_cold_layout(row_end, src, hot_mb)
     n_cold = len(zsrc) - H
-    streams, NB, S, seg, Nh, is_hub = split(row_end, gid, H, n_cold, min_indeg, bs, nb_max, seg_values)
+    streams, NB, S, seg, vbase, is_hub = split(row_end, gid, H, n_cold, min_indeg, bs, nb_max, seg_values)
     # every edge lands in exactly one stream
-    all_e = np.concatenate([sel for _, sel in streams.values()])
+    all_e = np.concatenate([sel for _, sel, _ in streams.values()])
     assert len(all_e) == len(src) and np.array_equal(np.sort(all_e), np.arange(len(src)))
-    for name_s, (re, sel) in streams.items():
+    for name_s, (re, sel, _) in streams.items():
         assert int(re[-1]) == len(sel), name_s
-    assert NB + S <= 255 and len(streams["cold"][1]) > 0
+    assert S <= 255 - NB and NB + S < KEY_MAIN and len(streams["cold"][1]) > 0
+    assert streams["cold"][2] == vbase[NB] and len(streams["cold"][0]) == vbase[NB + S] - vbase[NB]
     if case == "one_value_segments":
         assert S == n_cold
     if case == "one_value_raised_to_the_cap":
@@ -126,10 +135,10 @@ def test_three_way_split(case):
     x = np.random.default_rng(3).integers(1, 1000, len(row_end)).astype(np.int64)
     vals = x[src]
     want = direct_sums(row_end, vals)
-    assert sweep_and_combine(streams, vals, NB, S, Nh, is_hub) == want
+    assert sweep_and_combine(streams, vals, NB, S, vbase, is_hub) == want
     # and a missing cold-segment partial is seen
     in_last = (gid[streams["cold"][1]] - H) // seg == S - 1
-    assert (sweep_and_combine(streams, vals, NB, S, Nh, is_hub, drop_last_segment=True) != want) == bool(in_last.any())
+    assert (sweep_and_combine(streams, vals, NB, S, vbase, is_hub, drop_last_segment=True) != want) == bool(in_last.any())
 
 
 @pytest.mark.parametrize("hot_mb", [0.004, 24.0])

@@ -2,12 +2,13 @@
 panel.cuh), checked against per-vertex sums computed directly from the CSC:
 
   * hubs (in-degree >= D) ordered by in-degree, descending, ties by ascending id        (hub_order_key_kernel + sort)
-  * hub prefix N_b of every hot source block: all hubs for the first nb0 blocks (tier 0); for a later block b, the hubs
-    of in-degree d with d * m_b >= K, m_b = (edges block b -> hubs) / (edges into hubs), capped by N_{b-1}; trailing
-    blocks with N_b = 0 are dropped                                                    (build_panel_layout)
+  * hub prefix N_b of every hot source block, from the histogram of one keying with every block over every hub: all
+    hubs for the first nb0 blocks (tier 0); for a later block b, the hubs of in-degree d with d * m_b >= K, m_b =
+    (edges block b -> hubs) / (edges into hubs), capped by N_{b-1}; trailing blocks with N_b = 0 are dropped; the
+    edges are keyed again only when a prefix changed                                    (build_panel_layout)
   * edge keys: (hot source of block b -> hub h < N_b) = b, the rest main; a stable sort by hub position, then one by
-    key, lists every block's edges by virtual vertex vbase[b] + h (vbase[b] = sum of N_b' for b' < b) and the main
-    edges in CSC order; main in-degree = in-degree minus the panel coverage        (hub_key_kernel, panel_fill_kernel)
+    key, lists every block's edges by slot vbase[b] + h (vbase[b] = sum of N_b' for b' < b) and the main edges in CSC
+    order; main in-degree = in-degree minus the panel coverage                     (hub_key_kernel, group_fill_kernel)
   * each stream swept by the flagged-stream model of test_seg_model.py; hubs = main raw sum + the partials of blocks
     b = 0, 1, ... while h < N_b                                                        (combine_hub_kernel)
 Integer edge values make every summation order exact, so the comparison is bit-exact."""
