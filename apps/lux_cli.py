@@ -5,6 +5,8 @@
   python apps/lux_cli.py sssp       -ng 1 -file g.lux -start 0 [-check]            # sssp/sssp.cc
   python apps/lux_cli.py sssp       -weighted -file w.lux -start 0 [-check]        # weighted SSSP (i32 weight trailer; ours)
   python apps/lux_cli.py colfilter  -ng 1 -ni 10 -file ratings.lux                 # col_filter/colfilter.cc:85-107
+  python apps/lux_cli.py bc         -ng 1 -file g.lux [-start v | -nsrc K -seed S] [-out scores.npy] [-verbose]
+                                                                                   # betweenness centrality (ours)
   python apps/lux_cli.py converter  -nv N -ne M -input edges.txt -output g.lux     # tools/converter.cc:13-39 (host only)
 
 `-ll:gpu N` is accepted as a synonym of `-ng N` (README.md:47); -ll:fsize / -ll:zsize are accepted and ignored (HBM is
@@ -12,6 +14,12 @@ managed by the library).  With -ng > 1 the driver re-launches itself under torch
 Prints the reference's lines: "[Memory Setting] Set ll:fsize >= %zuMB and ll:zsize >= %zuMB" (pagerank.cc:84-85,
 components.cc:87-88), "ELAPSED TIME = %7.7f s" (pagerank.cc:118), "[PASS]/[FAIL] Check task: rowLeft(%u)
 numMistakes(%u)" (components_gpu.cu:831-836).  `-out file.npy` additionally saves the vertex values (the reference never writes its results anywhere, SURVEY §5).
+
+`bc` (no reference counterpart) sums Brandes' dependencies over a list of sources into f64 scores, not normalised.  The
+sources: `-start v` alone is the single source v; `-nsrc K` takes K distinct vertices
+numpy.random.default_rng(S).choice(nv, K, replace=False) with `-seed S` (default 0); neither flag means every vertex
+(exact BC).  It prints "ELAPSED TIME" (device time of the BC run) and no "[Memory Setting]" line: the reference has no
+formula for BC.
 """
 import os
 import subprocess
@@ -22,11 +30,12 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-APPS = {"pagerank": 0, "components": 1, "sssp": 2, "colfilter": 3}
+APPS = {"pagerank": 0, "components": 1, "sssp": 2, "colfilter": 3, "bc": 5}
 
 
 def parse(argv):
-    opt = dict(ng=1, ni=10, file=None, start=0, verbose=False, check=False, out=None, weighted=False)
+    opt = dict(ng=1, ni=10, file=None, start=0, verbose=False, check=False, out=None, weighted=False, start_set=False, nsrc=None,
+               seed=0)
     i = 0
     while i < len(argv):
         a = argv[i]
@@ -37,7 +46,11 @@ def parse(argv):
         elif a == "-file":
             opt["file"] = argv[i + 1]; i += 1
         elif a == "-start":
-            opt["start"] = int(argv[i + 1]); i += 1
+            opt["start"] = int(argv[i + 1]); opt["start_set"] = True; i += 1
+        elif a == "-nsrc":
+            opt["nsrc"] = int(argv[i + 1]); i += 1
+        elif a == "-seed":
+            opt["seed"] = int(argv[i + 1]); i += 1
         elif a == "-out":
             opt["out"] = argv[i + 1]; i += 1
         elif a in ("-verbose", "-v"):
@@ -75,6 +88,16 @@ def memory_setting(app, nv, ne, bounds, frontier_bytes, weighted=False):
     else:
         zc = ne * V + nv * E + nv * 2 * VTX + frontier_bytes * 2 + nv * 8 + max_edges * 4 + ne * W
     return max_fb // 1024 // 1024 + 1, zc // 1024 // 1024 + 1
+
+
+def bc_sources(opt, nv):
+    """The sources of `bc`: -nsrc K -> numpy.random.default_rng(seed).choice(nv, K, replace=False); -start v -> [v];
+    otherwise every vertex."""
+    if opt["nsrc"] is not None:
+        return np.random.default_rng(opt["seed"]).choice(nv, opt["nsrc"], replace=False).astype(np.uint32)
+    if opt["start_set"]:
+        return np.array([opt["start"]], np.uint32)
+    return np.arange(nv, dtype=np.uint32)
 
 
 def converter(argv):
@@ -128,13 +151,15 @@ def main():
     g = L.LuxGraph.from_file(opt["file"], app=L.APP_SSSP_WEIGHTED if weighted else APPS[app], rank=rank, nranks=world, device=local,
                              start=opt["start"], verbose=opt["verbose"])
     b = g.bounds()
-    if rank == 0:
+    if rank == 0 and app != "bc":
         fb, zc = memory_setting(app, g.nv, g.ne, b, int(b["fq_right"][-1]) + 1, weighted)
         print("[Memory Setting] Set ll:fsize >= %dMB and ll:zsize >= %dMB" % (fb, zc), flush=True)
     g.comm_init_torch()
     g.init()
     if app in ("pagerank", "colfilter"):
         g.iterate(opt["ni"])
+    elif app == "bc":
+        g.bc_run(bc_sources(opt, g.nv))
     else:
         g.run_to_convergence()
     if rank == 0:

@@ -49,7 +49,9 @@ typedef enum {
   LUXB_CC = 1,       /* components/ — push/pull hybrid, u32 label, max */
   LUXB_SSSP = 2,     /* sssp/       — push/pull hybrid, u32 hop distance, min(+1), INF = nv */
   LUXB_COLFILTER = 3, /* col_filter/ — pull model, float[20] vertex value */
-  LUXB_SSSP_WEIGHTED = 4 /* weighted SSSP (no reference counterpart) — push/pull hybrid, u32 distance, INF = LUXB_DIST_INF */
+  LUXB_SSSP_WEIGHTED = 4, /* weighted SSSP (no reference counterpart) — push/pull hybrid, u32 distance, INF = LUXB_DIST_INF */
+  LUXB_BC = 5            /* betweenness centrality (no reference counterpart) — Brandes over the SSSP engine's hop levels,
+                            f64 score per vertex; runs through luxb_bc_run */
 } luxb_app;
 
 /* Weighted SSSP (LUXB_SSSP_WEIGHTED):
@@ -65,6 +67,21 @@ typedef enum {
  *  - luxb_check counts the in-edges with D[u] != INF && D[v] > sat_add(D[u], w).
  * LUXB_SSSP keeps its hop-count semantics even when the CSC passed to it carries weights. */
 #define LUXB_DIST_INF 0xFFFFFFFFu
+
+/* Betweenness centrality (LUXB_BC).  The graph is the CSC's directed edges u -> v, one per in-edge of v; paths are
+ * unweighted (weights are ignored).  For a source s:
+ *  - lev[v] is the hop distance exactly as LUXB_SSSP computes it; INF = nv for unreachable vertices;
+ *  - sigma[s] = 1; every other sigma[v] = sum of sigma[u] over the in-edges (u, v) with lev[u] = lev[v] - 1 (fp64).
+ *    Parallel edges count with their multiplicity; a self-loop never matches;
+ *  - delta[v] = sigma[v] * sum of t[w] over the out-edges (v, w) with lev[w] = lev[v] + 1, t[w] = (1 + delta[w]) / sigma[w];
+ *  - unreachable vertices have sigma = delta = 0.
+ * For a list of sources S: BC[v] = sum over s in S, s != v, of delta_s(v), in fp64, not normalised; a source listed twice
+ * counts twice.  S = all vertices gives exact directed BC, a sample the usual estimate; on a graph stored with both
+ * directions of every edge the scores are twice the undirected BC.
+ * A BC handle's values (luxb_get_values / luxb_set_values and the _local_ variants) are the scores, 8 bytes per vertex.
+ * luxb_iterate, luxb_run_to_convergence and luxb_check return LUXB_ERR_ARG on it.  luxb_stats: iterations /
+ * pull_iterations = BFS iterations summed over sources, edges_processed = BFS scans + sigma edges + delta edges,
+ * loop_seconds = device time of the luxb_bc_run calls.  luxb_trace holds the BFS trace of the last source only. */
 
 typedef enum {
   LUXB_EXCHANGE_NCCL = 0, /* library collectives only: PageRank packs its share and broadcasts the two ranges of every
@@ -179,7 +196,7 @@ int luxb_iterate(luxb_graph* g, int iters, uint64_t* active_out);
 int luxb_run_to_convergence(luxb_graph* g, int max_iters, int* iters_out);
 
 /* ---- results / check / stats -------------------------------------------------------------------------------- */
-/* Full vertex-value array (what the reference holds in dist_lr[iter%2]): nv * {4 | 4 | 80} bytes.  PageRank on
+/* Full vertex-value array (what the reference holds in dist_lr[iter%2]): nv * {4 | 4 | 80 | 8 (BC scores)} bytes.  PageRank on
  * nranks > 1 exchanges only the values that are ever gathered each iteration and completes the full array on demand:
  * there the call is collective (every rank calls it at the same point). */
 int luxb_get_values(luxb_graph* g, void* host_out, size_t bytes);
@@ -242,6 +259,15 @@ int luxb_device_view_get(luxb_graph* g, luxb_device_view* out);
 
 /* Copy this rank's CSC slice back to host (tests: generator parity).  Arrays sized from luxb_device_view. */
 int luxb_get_local_csc(luxb_graph* g, luxb_eid* row_end_abs, luxb_vid* src, int32_t* weight);
+
+/* ---- betweenness centrality (LUXB_BC handles) -------------------------------------------------------------------- */
+/* Process the sources in order and add each source's delta into the handle's scores.  Collective on nranks > 1: every rank
+ * passes the same list.  Every source is validated before any work starts: a source >= nv returns LUXB_ERR_ARG and leaves
+ * the scores unchanged.  n_sources == 0 is a no-op.  LUXB_ERR_STATE before luxb_init, LUXB_ERR_ARG on another app. */
+int luxb_bc_run(luxb_graph* g, const luxb_vid* sources, int n_sources);
+/* The full lev / sigma / delta arrays (nv_count == nv entries each) of the last source processed; a NULL pointer skips that
+ * array.  Every rank holds them complete: not collective.  LUXB_ERR_STATE before the first source. */
+int luxb_bc_source_state(luxb_graph* g, uint32_t* lev, double* sigma, double* delta, size_t nv_count);
 
 void luxb_close(luxb_graph* g);
 const char* luxb_last_error(void);

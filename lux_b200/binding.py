@@ -6,7 +6,7 @@ import numpy as np
 
 from . import build as _build
 
-APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED = 0, 1, 2, 3, 4
+APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC = 0, 1, 2, 3, 4, 5
 DIST_INF = 0xFFFFFFFF  # APP_SSSP_WEIGHTED: distance of an unreachable vertex (LUXB_DIST_INF)
 EXCHANGE_NCCL, EXCHANGE_P2P, EXCHANGE_P2P_FUSED = 0, 1, 2
 DENSE_BITMAP, SPARSE_QUEUE = 0x1234567, 0x7654321
@@ -120,7 +120,7 @@ def convert_edgelist(edge_list_path, lux_path, nv, ne):
 
 
 _VDTYPE = {APP_PAGERANK: np.float32, APP_CC: np.uint32, APP_SSSP: np.uint32, APP_COLFILTER: np.float32,
-           APP_SSSP_WEIGHTED: np.uint32}
+           APP_SSSP_WEIGHTED: np.uint32, APP_BC: np.float64}
 
 
 class LuxGraph:
@@ -307,6 +307,24 @@ class LuxGraph:
         p = np.zeros(max_entries, np.int32)
         n = _chk(load_library().luxb_trace(self._h, _p(a), _p(p), C.c_int(max_entries)), "luxb_trace")
         return a[:n].copy(), p[:n].copy()
+
+    def bc_run(self, sources):
+        """Betweenness centrality (APP_BC handles): add the dependencies of every source, in order, to the scores that
+        values() returns.  Collective on nranks > 1 (every rank passes the same sources)."""
+        s = np.ascontiguousarray(np.asarray(sources, dtype=np.int64).reshape(-1))
+        if s.size and (s.min() < 0 or s.max() > 0xFFFFFFFF):
+            raise LuxError("luxb_bc_run failed: source out of the u32 range")
+        s = s.astype(np.uint32)
+        _chk(load_library().luxb_bc_run(self._h, _p(s) if s.size else None, C.c_int(len(s))), "luxb_bc_run")
+
+    def bc_source_state(self):
+        """(lev u32 [nv], sigma f64 [nv], delta f64 [nv]) of the last source processed by bc_run."""
+        lev = np.empty(self.nv, np.uint32)
+        sigma = np.empty(self.nv, np.float64)
+        delta = np.empty(self.nv, np.float64)
+        _chk(load_library().luxb_bc_source_state(self._h, _p(lev), _p(sigma), _p(delta), C.c_size_t(self.nv)),
+             "luxb_bc_source_state")
+        return lev, sigma, delta
 
     def enable_kernel_timing(self, on=True):
         _chk(load_library().luxb_enable_kernel_timing(self._h, C.c_int(1 if on else 0)), "luxb_enable_kernel_timing")

@@ -15,7 +15,7 @@ typedef struct ncclComm* ncclComm_t;
 typedef struct { char internal[128]; } ncclUniqueId;
 typedef enum { ncclSuccess = 0 } ncclResult_t;
 // values from nccl.h (stable across NCCL 2.x)
-enum { ncclInt8 = 0, ncclUint8 = 1, ncclInt32 = 2, ncclUint32 = 3, ncclInt64 = 4, ncclUint64 = 5, ncclFloat32 = 7 };
+enum { ncclInt8 = 0, ncclUint8 = 1, ncclInt32 = 2, ncclUint32 = 3, ncclInt64 = 4, ncclUint64 = 5, ncclFloat32 = 7, ncclFloat64 = 8 };
 enum { ncclSum = 0 };
 
 struct NcclApi {

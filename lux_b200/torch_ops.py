@@ -1,4 +1,4 @@
-"""PyTorch front-end of the C ABI (SURVEY §8 f4): the four Lux apps and weighted SSSP as `torch.ops.luxb.*` custom ops taking the CSC as
+"""PyTorch front-end of the C ABI (SURVEY §8 f4): the four Lux apps, weighted SSSP and betweenness centrality as `torch.ops.luxb.*` custom ops taking the CSC as
 torch tensors and returning torch tensors.  Plumbing only — every op opens a libluxb handle through the ctypes binding
 (lux_b200/binding.py), runs the app on the CUDA device of the current torch context and copies the result back; no torch
 kernel takes part in the computation, and there is no CPU fallback (the ops raise without a GPU).
@@ -9,7 +9,8 @@ kernel takes part in the computation, and there is no CPU fallback (the ops rais
     dist   = torch.ops.luxb.sssp(row_end, src, 0)               # i64 [nv]  (hop count, INF = nv, sssp_gpu.cu:122)
     x      = torch.ops.luxb.colfilter(row_end, src, weight, 10) # f32 [nv, 20]
     dist   = torch.ops.luxb.sssp_weighted(row_end, src, weight, 0)  # i64 [nv]  (weighted distance, INF = 2^32 - 1)
-row_end: int64 [nv] END offsets (the .lux convention); src: int64/int32 [ne]; weight: int32 [ne]."""
+    bc     = torch.ops.luxb.betweenness(row_end, src, sources)  # f64 [nv]  (Σ over sources of Brandes' δ, not normalised)
+row_end: int64 [nv] END offsets (the .lux convention); src: int64/int32 [ne]; weight: int32 [ne]; sources: int64/int32 [k] vertex ids."""
 import numpy as np
 import torch
 
@@ -30,6 +31,7 @@ _lib.define("components(Tensor row_end, Tensor src) -> Tensor")
 _lib.define("sssp(Tensor row_end, Tensor src, int start) -> Tensor")
 _lib.define("colfilter(Tensor row_end, Tensor src, Tensor weight, int num_iter) -> Tensor")
 _lib.define("sssp_weighted(Tensor row_end, Tensor src, Tensor weight, int start) -> Tensor")
+_lib.define("betweenness(Tensor row_end, Tensor src, Tensor sources) -> Tensor")
 
 
 def _pagerank(row_end, src, num_iter):
@@ -59,6 +61,11 @@ def _sssp_weighted(row_end, src, weight, start):
     return torch.from_numpy(out["labels"].astype(np.int64)).to(row_end.device)
 
 
+def _betweenness(row_end, src, sources):
+    out = _apps.betweenness(_np(row_end, np.uint64), _np(src, np.uint32), sources=_np(sources, np.int64), device=_device_index(row_end))
+    return torch.from_numpy(out).to(row_end.device)
+
+
 for _name, _fn in (("pagerank", _pagerank), ("components", _components), ("sssp", _sssp), ("colfilter", _colfilter),
-                   ("sssp_weighted", _sssp_weighted)):
+                   ("sssp_weighted", _sssp_weighted), ("betweenness", _betweenness)):
     _lib.impl(_name, _fn, "CompositeExplicitAutograd")
