@@ -7,6 +7,8 @@
   python apps/lux_cli.py colfilter  -ng 1 -ni 10 -file ratings.lux                 # col_filter/colfilter.cc:85-107
   python apps/lux_cli.py bc         -ng 1 -file g.lux [-start v | -nsrc K -seed S] [-out scores.npy] [-verbose]
                                                                                    # betweenness centrality (ours)
+  python apps/lux_cli.py bc         -weighted -file w.lux [-start v | -nsrc K -seed S] [-out scores.npy]
+                                                                                   # weighted BC (i32 trailer, w >= 1; ours)
   python apps/lux_cli.py converter  -nv N -ne M -input edges.txt -output g.lux     # tools/converter.cc:13-39 (host only)
 
 `-ll:gpu N` is accepted as a synonym of `-ng N` (README.md:47); -ll:fsize / -ll:zsize are accepted and ignored (HBM is
@@ -19,7 +21,8 @@ numMistakes(%u)" (components_gpu.cu:831-836).  `-out file.npy` additionally save
 sources: `-start v` alone is the single source v; `-nsrc K` takes K distinct vertices
 numpy.random.default_rng(S).choice(nv, K, replace=False) with `-seed S` (default 0); neither flag means every vertex
 (exact BC).  It prints "ELAPSED TIME" (device time of the BC run) and no "[Memory Setting]" line: the reference has no
-formula for BC.
+formula for BC.  `bc -weighted` reads the .lux i32 weight trailer and runs weighted BC (shortest paths by weighted
+distance, every weight >= 1) with the same source flags.
 """
 import os
 import subprocess
@@ -147,8 +150,9 @@ def main():
         import torch.distributed as dist
         torch.cuda.set_device(local)
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
-    weighted = opt["weighted"] and app == "sssp"  # weighted SSSP over the .lux i32 weight trailer
-    g = L.LuxGraph.from_file(opt["file"], app=L.APP_SSSP_WEIGHTED if weighted else APPS[app], rank=rank, nranks=world, device=local,
+    weighted = opt["weighted"] and app in ("sssp", "bc")  # weighted SSSP / BC over the .lux i32 weight trailer
+    weighted_app = {"sssp": L.APP_SSSP_WEIGHTED, "bc": L.APP_BC_WEIGHTED}
+    g = L.LuxGraph.from_file(opt["file"], app=weighted_app[app] if weighted else APPS[app], rank=rank, nranks=world, device=local,
                              start=opt["start"], verbose=opt["verbose"])
     b = g.bounds()
     if rank == 0 and app != "bc":

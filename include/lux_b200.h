@@ -50,8 +50,10 @@ typedef enum {
   LUXB_SSSP = 2,     /* sssp/       — push/pull hybrid, u32 hop distance, min(+1), INF = nv */
   LUXB_COLFILTER = 3, /* col_filter/ — pull model, float[20] vertex value */
   LUXB_SSSP_WEIGHTED = 4, /* weighted SSSP (no reference counterpart) — push/pull hybrid, u32 distance, INF = LUXB_DIST_INF */
-  LUXB_BC = 5            /* betweenness centrality (no reference counterpart) — Brandes over the SSSP engine's hop levels,
+  LUXB_BC = 5,           /* betweenness centrality (no reference counterpart) — Brandes over the SSSP engine's hop levels,
                             f64 score per vertex; runs through luxb_bc_run */
+  LUXB_BC_WEIGHTED = 6   /* weighted betweenness centrality (no reference counterpart) — Brandes over the weighted SSSP
+                            distances (weights >= 1), f64 score per vertex; runs through luxb_bc_run */
 } luxb_app;
 
 /* Weighted SSSP (LUXB_SSSP_WEIGHTED):
@@ -83,6 +85,25 @@ typedef enum {
  * pull_iterations = BFS iterations summed over sources, edges_processed = BFS scans + sigma edges + delta edges,
  * loop_seconds = device time of the luxb_bc_run calls.  luxb_trace holds the BFS trace of the last source only. */
 
+/* Weighted betweenness centrality (LUXB_BC_WEIGHTED).  The graph is the CSC's directed edges u -> v with their i32
+ * weights w, and every weight must be >= 1: a smaller one fails the open with LUXB_ERR_ARG (checked on the device).  With
+ * w >= 1 every shortest-path edge goes to a strictly larger distance, so ascending distances order the shortest-path DAG;
+ * a zero weight would put DAG edges inside one distance and a zero-weight cycle would make sigma unbounded.  The graph
+ * must carry weights (csc->weight, or the .lux i32 trailer); luxb_open_rmat generates the [1, 255] weights of weighted
+ * SSSP.  For a source s:
+ *  - D[v] is the distance exactly as LUXB_SSSP_WEIGHTED computes it (u32, sat_add, INF = LUXB_DIST_INF: a path whose
+ *    sum would reach 2^32 - 1 counts as unreachable);
+ *  - an edge (u, v, w) is tight iff D[v] != INF and (uint64)D[u] + w == D[v], in 64 bits: an unreached u never matches,
+ *    and neither does an edge whose sum saturates to INF;
+ *  - sigma[s] = 1; every other sigma[v] = sum of sigma[u] over the tight in-edges of v (fp64).  Parallel edges count
+ *    with their multiplicity, but only those at the minimal weight are tight; a self-loop is never tight;
+ *  - delta[v] = sigma[v] * sum of t[x] over the tight out-edges (v, x), t[x] = (1 + delta[x]) / sigma[x];
+ *  - unreachable vertices have sigma = delta = 0.
+ * Scores accumulate as for LUXB_BC (sum over s in S, s != v, fp64, not normalised, repeats count).  Unit weights give
+ * LUXB_BC exactly: D = lev, and sigma, delta and the scores are bit for bit equal.  luxb_bc_source_state returns D as
+ * `lev`.  Values, luxb_iterate / luxb_run_to_convergence / luxb_check, luxb_stats and the phase timing behave as for
+ * LUXB_BC; luxb_trace holds the weighted SSSP trace of the last source. */
+
 typedef enum {
   LUXB_EXCHANGE_NCCL = 0, /* library collectives only: PageRank packs its share and broadcasts the two ranges of every
                              owner (grouped ncclBroadcast); CC / SSSP broadcast frontier slots and label slices;
@@ -104,7 +125,7 @@ typedef struct {
   luxb_eid ne;
   const luxb_eid* row_end;
   const luxb_vid* src;
-  const int32_t* weight; /* needed by LUXB_COLFILTER and LUXB_SSSP_WEIGHTED; ignored by the other apps */
+  const int32_t* weight; /* needed by LUXB_COLFILTER, LUXB_SSSP_WEIGHTED and LUXB_BC_WEIGHTED; ignored by the others */
 } luxb_csc;
 
 typedef struct {
@@ -136,7 +157,8 @@ int luxb_open_file(const char* lux_path, const luxb_config* cfg, luxb_graph** ou
 /* Synthetic inputs generated ON THE DEVICE (no reference counterpart; SURVEY §8d): deterministic counter-based
  * RMAT (a,b,c,d = .57,.19,.19,.05), endpoints >= nv rejected, canonical (dst,src)-sorted CSC.  Bit-identical to
  * oracle lo_gen_rmat_csc.  Every rank generates the edge stream and keeps only its own partition.
- * app == LUXB_SSSP_WEIGHTED: every edge also gets a directed weight in [1, 255] that depends only on (seed, src, dst):
+ * app == LUXB_SSSP_WEIGHTED or LUXB_BC_WEIGHTED: every edge also gets a directed weight in [1, 255] that depends only on
+ * (seed, src, dst):
  *   w = 1 + (splitmix64(splitmix64(seed ^ 0x9E3779B97F4A7C15) ^ (dst << 32 | src)) >> 32) % 255
  * (bit-identical to the weighted-SSSP test oracle, tests/weighted_oracle.c wo_rmat_weight). */
 int luxb_open_rmat(int scale, luxb_vid nv, luxb_eid ne, uint64_t seed, const luxb_config* cfg, luxb_graph** out);
@@ -260,13 +282,13 @@ int luxb_device_view_get(luxb_graph* g, luxb_device_view* out);
 /* Copy this rank's CSC slice back to host (tests: generator parity).  Arrays sized from luxb_device_view. */
 int luxb_get_local_csc(luxb_graph* g, luxb_eid* row_end_abs, luxb_vid* src, int32_t* weight);
 
-/* ---- betweenness centrality (LUXB_BC handles) -------------------------------------------------------------------- */
+/* ---- betweenness centrality (LUXB_BC and LUXB_BC_WEIGHTED handles) ------------------------------------------------ */
 /* Process the sources in order and add each source's delta into the handle's scores.  Collective on nranks > 1: every rank
  * passes the same list.  Every source is validated before any work starts: a source >= nv returns LUXB_ERR_ARG and leaves
  * the scores unchanged.  n_sources == 0 is a no-op.  LUXB_ERR_STATE before luxb_init, LUXB_ERR_ARG on another app. */
 int luxb_bc_run(luxb_graph* g, const luxb_vid* sources, int n_sources);
-/* The full lev / sigma / delta arrays (nv_count == nv entries each) of the last source processed; a NULL pointer skips that
- * array.  Every rank holds them complete: not collective.  LUXB_ERR_STATE before the first source. */
+/* The full lev / sigma / delta arrays (nv_count == nv entries each) of the last source processed (LUXB_BC_WEIGHTED: lev
+ * is the u32 distance D); a NULL pointer skips that array.  Every rank holds them complete: not collective.  LUXB_ERR_STATE before the first source. */
 int luxb_bc_source_state(luxb_graph* g, uint32_t* lev, double* sigma, double* delta, size_t nv_count);
 
 void luxb_close(luxb_graph* g);

@@ -4,12 +4,13 @@ pagerank   : pagerank/pagerank.cc:105-118     (-ni fixed iterations)
 components : components/components.cc:108-135 (run until no partition reports an active vertex)
 sssp       : sssp/sssp.cc                     (same loop, -start; with weights: weighted SSSP, ours)
 colfilter  : col_filter/colfilter.cc:71-81    (-ni fixed iterations)
-betweenness: Brandes from a list of sources over the SSSP engine's hop levels (ours; the reference has no BC)
+betweenness: Brandes from a list of sources over the SSSP engine's hop levels, or with weights over the weighted
+             SSSP distances (ours; the reference has no BC)
 Single-rank convenience wrappers; multi-GPU callers drive LuxGraph directly (see bench.py).
 """
 import numpy as np
 
-from .binding import LuxGraph, APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC
+from .binding import LuxGraph, APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC, APP_BC_WEIGHTED
 
 
 def pagerank(row_end, src, num_iter=10, device=0):
@@ -50,13 +51,15 @@ def colfilter(row_end, src, weight, num_iter=10, device=0):
         return g.values()
 
 
-def betweenness(row_end, src, sources=None, device=0):
-    """Betweenness centrality scores (f64 [nv], not normalised) over the CSC's directed edges, unweighted: the sum over
-    the sources s != v of Brandes' dependency delta_s(v).  sources=None means every vertex (exact BC); a sample gives the
-    usual estimate, a source listed twice counts twice."""
+def betweenness(row_end, src, sources=None, device=0, weight=None):
+    """Betweenness centrality scores (f64 [nv], not normalised) over the CSC's directed edges: the sum over the sources
+    s != v of Brandes' dependency delta_s(v).  Unweighted paths, or with `weight` (i32 per edge, CSC order, every weight
+    >= 1) shortest paths by weighted distance, where only the edges on a shortest path count.  sources=None means every
+    vertex (exact BC); a sample gives the usual estimate, a source listed twice counts twice."""
     nv = len(row_end)
     srcs = np.arange(nv, dtype=np.uint32) if sources is None else np.asarray(sources)
-    with LuxGraph.from_csc(row_end, src, app=APP_BC, device=device) as g:
+    app = APP_BC if weight is None else APP_BC_WEIGHTED
+    with LuxGraph.from_csc(row_end, src, weight, app=app, device=device) as g:
         g.init()
         g.bc_run(srcs)
         return g.values()

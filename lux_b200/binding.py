@@ -6,8 +6,8 @@ import numpy as np
 
 from . import build as _build
 
-APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC = 0, 1, 2, 3, 4, 5
-DIST_INF = 0xFFFFFFFF  # APP_SSSP_WEIGHTED: distance of an unreachable vertex (LUXB_DIST_INF)
+APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC, APP_BC_WEIGHTED = 0, 1, 2, 3, 4, 5, 6
+DIST_INF = 0xFFFFFFFF  # APP_SSSP_WEIGHTED / APP_BC_WEIGHTED: distance of an unreachable vertex (LUXB_DIST_INF)
 EXCHANGE_NCCL, EXCHANGE_P2P, EXCHANGE_P2P_FUSED = 0, 1, 2
 DENSE_BITMAP, SPARSE_QUEUE = 0x1234567, 0x7654321
 CF_K = 20
@@ -120,7 +120,7 @@ def convert_edgelist(edge_list_path, lux_path, nv, ne):
 
 
 _VDTYPE = {APP_PAGERANK: np.float32, APP_CC: np.uint32, APP_SSSP: np.uint32, APP_COLFILTER: np.float32,
-           APP_SSSP_WEIGHTED: np.uint32, APP_BC: np.float64}
+           APP_SSSP_WEIGHTED: np.uint32, APP_BC: np.float64, APP_BC_WEIGHTED: np.float64}
 
 
 class LuxGraph:
@@ -309,8 +309,9 @@ class LuxGraph:
         return a[:n].copy(), p[:n].copy()
 
     def bc_run(self, sources):
-        """Betweenness centrality (APP_BC handles): add the dependencies of every source, in order, to the scores that
-        values() returns.  Collective on nranks > 1 (every rank passes the same sources)."""
+        """Betweenness centrality (APP_BC handles, or APP_BC_WEIGHTED over weighted shortest paths, weights >= 1): add
+        the dependencies of every source, in order, to the scores that values() returns.  Collective on nranks > 1 (every
+        rank passes the same sources)."""
         s = np.ascontiguousarray(np.asarray(sources, dtype=np.int64).reshape(-1))
         if s.size and (s.min() < 0 or s.max() > 0xFFFFFFFF):
             raise LuxError("luxb_bc_run failed: source out of the u32 range")
@@ -318,7 +319,8 @@ class LuxGraph:
         _chk(load_library().luxb_bc_run(self._h, _p(s) if s.size else None, C.c_int(len(s))), "luxb_bc_run")
 
     def bc_source_state(self):
-        """(lev u32 [nv], sigma f64 [nv], delta f64 [nv]) of the last source processed by bc_run."""
+        """(lev u32 [nv], sigma f64 [nv], delta f64 [nv]) of the last source processed by bc_run; on an APP_BC_WEIGHTED
+        handle lev is the weighted distance (INF = DIST_INF)."""
         lev = np.empty(self.nv, np.uint32)
         sigma = np.empty(self.nv, np.float64)
         delta = np.empty(self.nv, np.float64)

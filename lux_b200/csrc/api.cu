@@ -16,8 +16,14 @@
 #include "seg.cuh"
 #include "push.cuh"
 #include "runtime.cuh"
+#include <thrust/iterator/counting_iterator.h>
 
 using namespace luxb;
+// betweenness centrality, over hop levels or over weighted distance classes: luxb_bc_run instead of luxb_iterate
+static bool is_bc_app(luxb_app app) { return app == LUXB_BC || app == LUXB_BC_WEIGHTED; }
+// labels are weighted distances (u32, INF = LUXB_DIST_INF, label_iteration<WeightedDistProgram>): the app reads the CSC
+// weights, keeps out_w beside the push CSR and pulls through the merge-path sweep only
+static bool weighted_labels(luxb_app app) { return app == LUXB_SSSP_WEIGHTED || app == LUXB_BC_WEIGHTED; }
 static const char* const kPhaseName[12] = {"pull_tile", "fixup", "refresh", "rechunk", "barrier", "panel", "combine", "pack+push", "pull/bcast", "cold_hub", "bc_sigma", "bc_delta"};
 static void pt_mark(luxb_graph* g, int tag) {
   PhaseTimer& pt = g->pt;
@@ -32,7 +38,7 @@ static void pt_print(luxb_graph* g) {
   if (g->pt.on && g->pt.cnt) {
     char line[1024];
     // betweenness centrality times its two level sweeps per source (the BFS before them is not split)
-    const bool bc = g->cfg.app == LUXB_BC;
+    const bool bc = is_bc_app(g->cfg.app);
     int n = snprintf(line, sizeof(line), "[luxb rank %d] phase means over %ld %s:", g->cfg.rank, g->pt.cnt, bc ? "sources" : "iterations");
     double sum = 0;
     for (int k = bc ? 10 : 0; k < (bc ? 12 : 10); ++k) {
@@ -54,7 +60,7 @@ static void pt_flush(luxb_graph* g) {
     cudaEventElapsedTime(&ms, pt.ev[i - 1], pt.ev[i]);
     pt.sum[pt.tag[i]] += ms;
     // one PageRank iteration (its pull sweep), or one BC source (its σ sweep: the BFS's own pull sweeps also mark tag 0)
-    if (pt.tag[i] == (g->cfg.app == LUXB_BC ? 10 : 0)) pt.cnt++;
+    if (pt.tag[i] == (is_bc_app(g->cfg.app) ? 10 : 0)) pt.cnt++;
   }
   for (cudaEvent_t e : pt.ev) cudaEventDestroy(e);
   pt.ev.clear();
@@ -239,7 +245,7 @@ static bool use_balanced_split(const luxb_config* cfg) {
 
 static int check_config(const luxb_config* cfg) {
   LUXB_ARG(cfg != nullptr, "config is NULL");
-  LUXB_ARG(cfg->app >= LUXB_PAGERANK && cfg->app <= LUXB_BC, "unknown app %d", (int)cfg->app);
+  LUXB_ARG(cfg->app >= LUXB_PAGERANK && cfg->app <= LUXB_BC_WEIGHTED, "unknown app %d", (int)cfg->app);
   LUXB_ARG(cfg->nranks >= 1 && cfg->nranks <= LUXB_MAX_PARTS, "nranks %d out of range [1,%d]", cfg->nranks, LUXB_MAX_PARTS);
   LUXB_ARG(cfg->rank >= 0 && cfg->rank < cfg->nranks, "rank %d out of range", cfg->rank);
   return 0;
@@ -248,7 +254,7 @@ static int check_config(const luxb_config* cfg) {
 // the push/pull hybrid apps: u32 labels in one replica (d_val[0]), frontier engine, luxb_check
 static bool is_label_app(luxb_app app) { return app == LUXB_CC || app == LUXB_SSSP || app == LUXB_SSSP_WEIGHTED; }
 // apps that read the CSC's edge weights
-static bool uses_weights(luxb_app app) { return app == LUXB_COLFILTER || app == LUXB_SSSP_WEIGHTED; }
+static bool uses_weights(luxb_app app) { return app == LUXB_COLFILTER || weighted_labels(app); }
 
 static int graph_begin(const luxb_config* cfg, uint32_t nv, uint64_t ne, luxb_graph** out) {
   LUXB_TRY(check_config(cfg));
@@ -391,15 +397,18 @@ static int upload_slice(luxb_graph* g, const uint64_t* row_end_slice_abs, const 
   LUXB_CUDA(cudaMemcpyAsync(&bad, d_bad, 8, cudaMemcpyDeviceToHost, g->stream));
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
   unsigned long long neg = 0;
-  if (g->cfg.app == LUXB_SSSP_WEIGHTED && g->e_part) {  // shortest paths need w >= 0 (checked the same way, on the device)
+  const bool bc = g->cfg.app == LUXB_BC_WEIGHTED;
+  if (weighted_labels(g->cfg.app) && g->e_part) {  // shortest paths need w >= 0, BC w >= 1 (checked the same way, on the device)
     LUXB_CUDA(cudaMemsetAsync(d_bad, 0, 8, g->stream));
-    negative_weight_kernel<<<g->num_sms * 8, 256, 0, g->stream>>>(g->d_weight, g->e_part, d_bad);
+    if (bc) light_weight_kernel<<<g->num_sms * 8, 256, 0, g->stream>>>(g->d_weight, g->e_part, 1, d_bad);
+    else negative_weight_kernel<<<g->num_sms * 8, 256, 0, g->stream>>>(g->d_weight, g->e_part, d_bad);
     LUXB_CUDA(cudaMemcpyAsync(&neg, d_bad, 8, cudaMemcpyDeviceToHost, g->stream));
     LUXB_CUDA(cudaStreamSynchronize(g->stream));
   }
   LUXB_CUDA(cudaFree(d_tmp));
   LUXB_ARG(bad == 0, "%llu source ids of this rank's slice are >= nv (%u)", bad, g->nv);
-  LUXB_ARG(neg == 0, "%llu edge weights of this rank's slice are negative (weighted SSSP needs w >= 0)", neg);
+  LUXB_ARG(neg == 0 || bc, "%llu edge weights of this rank's slice are negative (weighted SSSP needs w >= 0)", neg);
+  LUXB_ARG(neg == 0, "%llu edge weights of this rank's slice are < 1 (weighted betweenness centrality needs w >= 1)", neg);
   return finish_layout(g);
 }
 
@@ -425,7 +434,8 @@ int luxb_open_csc(const luxb_csc* csc, const luxb_config* cfg, luxb_graph** out)
   LUXB_ARG(csc && csc->row_end && (csc->src || csc->ne == 0), "csc arrays are NULL");
   LUXB_TRY(check_config(cfg));
   LUXB_ARG(cfg->app != LUXB_COLFILTER || csc->weight, "col_filter needs edge weights (EDGE_WEIGHT, col_filter/app.h:22)");
-  LUXB_ARG(cfg->app != LUXB_SSSP_WEIGHTED || csc->weight || csc->ne == 0, "weighted SSSP needs edge weights");
+  LUXB_ARG(!weighted_labels(cfg->app) || csc->weight || csc->ne == 0, "%s needs edge weights",
+           cfg->app == LUXB_BC_WEIGHTED ? "weighted betweenness centrality" : "weighted SSSP");
   LUXB_TRY(validate_row_end(csc->nv, csc->ne, csc->row_end));
   luxb_graph* g = nullptr;
   int rc = open_host_begin(cfg, csc->nv, csc->ne, csc->row_end, &g);
@@ -866,7 +876,7 @@ static int build_push_csr(luxb_graph* g) {
   LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
     return cub::DeviceRadixSort::SortPairs(t, b, g->d_src, d_keys_out, d_dst, g->d_out_dst, (long long)g->e_part, 0, vbits, g->stream);
   }));
-  if (g->cfg.app == LUXB_SSSP_WEIGHTED) {
+  if (weighted_labels(g->cfg.app)) {
     // the weights in the same order: the same stable sort on the same keys applies the same permutation
     LUXB_TRY(dmalloc(&g->d_out_w, g->e_part));
     LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
@@ -913,7 +923,7 @@ static int reset_label_state(luxb_graph* g, bool all_active, uint32_t start) {
     if (cc) iota_kernel<<<grid, 256, 0, g->stream>>>(lab, g->nv);
     else {
       // INF: nv for hop counts (sssp_gpu.cu:733-744), LUXB_DIST_INF for weighted distances
-      fill_kernel<uint32_t><<<grid, 256, 0, g->stream>>>(lab, g->nv, g->cfg.app == LUXB_SSSP_WEIGHTED ? kDistInf : g->nv);
+      fill_kernel<uint32_t><<<grid, 256, 0, g->stream>>>(lab, g->nv, weighted_labels(g->cfg.app) ? kDistInf : g->nv);
       uint32_t zero = 0;
       if (start < g->nv)
         LUXB_CUDA(cudaMemcpyAsync(lab + start, &zero, 4, cudaMemcpyHostToDevice, g->stream));
@@ -1188,15 +1198,16 @@ int luxb_init(luxb_graph* g) {
     case LUXB_CC:
     case LUXB_SSSP:
     case LUXB_SSSP_WEIGHTED:
-    case LUXB_BC: {  // betweenness centrality: SSSP's state for the BFS of every source, then its own arrays (bc_alloc)
+    case LUXB_BC:
+    case LUXB_BC_WEIGHTED: {  // betweenness centrality: SSSP's state for the search of every source, then its own arrays (bc_alloc)
       g->vbytes = 4;
-      LUXB_ARG(g->cfg.app == LUXB_CC || g->cfg.app == LUXB_BC || g->cfg.start_vtx < g->nv, "start vertex %u >= nv", g->cfg.start_vtx);
+      LUXB_ARG(g->cfg.app == LUXB_CC || is_bc_app(g->cfg.app) || g->cfg.start_vtx < g->nv, "start vertex %u >= nv", g->cfg.start_vtx);
       LUXB_TRY(dmalloc((uint32_t**)&g->d_val[0], g->nv));
       LUXB_TRY(dmalloc(&g->d_cur, g->n_part));
       LUXB_TRY(build_push_csr(g));
       // hot-packed label copies for the pull sweeps (same layout as PageRank; refreshed before every pull sweep).
-      // Weighted SSSP pulls through the merge-path sweep only: the flagged streams carry no weights.
-      LUXB_TRY(build_gather_side(g, /*compact_cold=*/false, /*streams=*/g->cfg.app != LUXB_SSSP_WEIGHTED));
+      // Weighted distances are pulled through the merge-path sweep only: the flagged streams carry no weights.
+      LUXB_TRY(build_gather_side(g, /*compact_cold=*/false, /*streams=*/!weighted_labels(g->cfg.app)));
       g->big_capacity = (uint32_t)std::min<uint64_t>(g->e_part / kPushBigDegree + 1024, 0x7FFFFFFFull);
       LUXB_TRY(dmalloc((PushArgs::BigSeg**)&g->d_big_list, g->big_capacity));
       LUXB_TRY(dmalloc(&g->d_fq_all, g->fq_total));
@@ -1213,7 +1224,7 @@ int luxb_init(luxb_graph* g) {
         LUXB_TRY(allgather_slices(g, g->d_val[0], 4));
         LUXB_CUDA(cudaStreamSynchronize(g->stream));
       }
-      if (g->cfg.app == LUXB_BC) LUXB_TRY(bc_alloc(g));
+      if (is_bc_app(g->cfg.app)) LUXB_TRY(bc_alloc(g));
       break;
     }
   }
@@ -2433,7 +2444,7 @@ static int finish_timed(luxb_graph* g) {
 int luxb_iterate(luxb_graph* g, int iters, uint64_t* active_out) {
   LUXB_ARG(g != nullptr, "graph is NULL");
   if (!g->inited) { set_error("luxb_iterate before luxb_init"); return LUXB_ERR_STATE; }
-  LUXB_ARG(g->cfg.app != LUXB_BC, "luxb_iterate: betweenness centrality runs through luxb_bc_run");
+  LUXB_ARG(!is_bc_app(g->cfg.app), "luxb_iterate: betweenness centrality runs through luxb_bc_run");
   LUXB_ARG(iters >= 0, "negative iteration count");
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
   if (const char* env = getenv("LUXB_PHASE_TIMING")) { g->pt.on = atoi(env) != 0; g->pt.per_call = atoi(env) == 2; }  // may change between calls
@@ -2450,7 +2461,7 @@ int luxb_iterate(luxb_graph* g, int iters, uint64_t* active_out) {
 int luxb_run_to_convergence(luxb_graph* g, int max_iters, int* iters_out) {
   LUXB_ARG(g != nullptr, "graph is NULL");
   if (!g->inited) { set_error("luxb_run_to_convergence before luxb_init"); return LUXB_ERR_STATE; }
-  LUXB_ARG(g->cfg.app != LUXB_BC, "luxb_run_to_convergence: betweenness centrality runs through luxb_bc_run");
+  LUXB_ARG(!is_bc_app(g->cfg.app), "luxb_run_to_convergence: betweenness centrality runs through luxb_bc_run");
   LUXB_ARG(is_label_app(g->cfg.app), "only push apps converge (pagerank/col_filter run -ni iterations)");
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
   LUXB_CUDA(cudaEventRecord(g->ev_begin, g->stream));
@@ -2490,8 +2501,14 @@ static int bc_alloc(luxb_graph* g) {
   LUXB_CUDA(cudaMemsetAsync(g->d_scores, 0, (size_t)g->nv * 8, g->stream));
   cub::DoubleBuffer<uint32_t> keys(nullptr, nullptr), vals(nullptr, nullptr);
   LUXB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, g->bc_sort_bytes, keys, vals, (int)g->nv, 0, 32, g->stream));
+  if (g->cfg.app == LUXB_BC_WEIGHTED) {  // the class heads are selected with the same temporary storage after the sort
+    size_t sel = 0;
+    LUXB_CUDA(cub::DeviceSelect::If(nullptr, sel, thrust::counting_iterator<uint32_t>(0), (uint32_t*)nullptr, (uint32_t*)nullptr,
+                                    (int)g->nv, BcClassHead{nullptr}, g->stream));
+    g->bc_sort_bytes = std::max(g->bc_sort_bytes, sel);
+  }
   LUXB_TRY(dmalloc((char**)&g->d_bc_sort_tmp, g->bc_sort_bytes));
-  LUXB_TRY(dmalloc(&g->d_bc_ctl, 4));
+  LUXB_TRY(dmalloc(&g->d_bc_ctl, 5));
   LUXB_TRY(dmalloc(&g->d_bc_hubs, g->e_part / kBcSegment + 1));
   LUXB_TRY(dmalloc(&g->d_bc_partial, 2 * (g->e_part / kBcSegment) + 2));
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
@@ -2500,7 +2517,8 @@ static int bc_alloc(luxb_graph* g) {
 }
 
 extern "C++" {
-// the sum of f(neighbour) over the edge lists of n level vertices into out[0, n): main sweep, hub segments, combine
+// the sum of f(neighbour) over the edge lists of n level vertices into out[0, n): main sweep, hub segments, combine.
+// Hop levels keep the neighbours on level `target`; distance classes keep the tight edges
 template <bool kOut>
 static int bc_level_sum(luxb_graph* g, const uint32_t* order, uint32_t n, uint32_t target, double* out) {
   if (n == 0) return 0;
@@ -2520,8 +2538,15 @@ static int bc_level_sum(luxb_graph* g, const uint32_t* order, uint32_t n, uint32
   a.partial = g->d_bc_partial;
   a.edges = g->d_counters;
   LUXB_CUDA(cudaMemsetAsync(a.ctl, 0, sizeof(BcCtl), g->stream));
-  bc_level_sum_kernel<kOut><<<grid_for(n, kBcThreads / 32, g->num_sms * 16), kBcThreads, 0, g->stream>>>(a);
-  bc_hub_segments_kernel<kOut><<<g->num_sms * 2, kBcThreads, 0, g->stream>>>(a);
+  const int grid = grid_for(n, kBcThreads / 32, g->num_sms * 16);
+  if (g->cfg.app == LUXB_BC_WEIGHTED) {  // distance classes: tight edges at each vertex's own distance, target unused
+    const BcClassArgs c{a, kOut ? g->d_out_w : g->d_weight};
+    bc_class_sum_kernel<kOut><<<grid, kBcThreads, 0, g->stream>>>(c);
+    bc_class_hub_segments_kernel<kOut><<<g->num_sms * 2, kBcThreads, 0, g->stream>>>(c);
+  } else {
+    bc_level_sum_kernel<kOut><<<grid, kBcThreads, 0, g->stream>>>(a);
+    bc_hub_segments_kernel<kOut><<<g->num_sms * 2, kBcThreads, 0, g->stream>>>(a);
+  }
   bc_combine_kernel<<<8, 128, 0, g->stream>>>(a.ctl, a.hubs, a.partial, out);
   LUXB_CUDA(cudaGetLastError());
   g->stats.kernel_launches += 3;
@@ -2576,17 +2601,75 @@ static int bc_levels(luxb_graph* g, uint32_t& L) {
   return 0;
 }
 
-// one source: BFS levels (the SSSP engine), level lists, forward σ, backward δ, scores += δ
+// the distance classes of the weighted distances in the replica: order[] sorted stably by distance, class_off (host
+// bc_off, C + 1 entries, one class per distinct distance) and, on several ranks, every partition's piece of every class.
+// The keys are sparse, so the class offsets are the positions where the sorted key changes.  The class count is only
+// known on the device: the host reads a bound on it (min(reached, largest distance + 1)) worth of offsets, padded with
+// empty classes, together with the count in one synchronisation.
+static int bc_classes(luxb_graph* g, uint32_t& C) {
+  const uint32_t nv = g->nv;
+  const uint32_t* dist = reinterpret_cast<const uint32_t*>(g->d_val[0]);
+  const int grid = g->num_sms * 8;
+  uint32_t* ctl = g->d_bc_ctl;
+  LUXB_CUDA(cudaMemsetAsync(ctl + 2, 0, 8, g->stream));
+  bc_dist_max_kernel<<<grid, 256, 0, g->stream>>>(dist, nv, ctl + 2);
+  uint32_t h[2] = {0, 0};
+  LUXB_CUDA(cudaMemcpyAsync(h, ctl + 2, 8, cudaMemcpyDeviceToHost, g->stream));
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  const uint32_t reached = h[1], K = h[0] + 1;  // K: the key of the unreached (<= 2^32 - 1: a distance is < INF)
+  int bits = 1;  // keys 0 .. K
+  while ((1ull << bits) <= K) ++bits;
+  uint32_t* k0 = reinterpret_cast<uint32_t*>(g->d_delta);
+  uint32_t* v0 = reinterpret_cast<uint32_t*>(g->d_sigma);
+  bc_dist_keys_kernel<<<grid, 256, 0, g->stream>>>(dist, nv, K, k0, v0);
+  cub::DoubleBuffer<uint32_t> keys(k0, k0 + nv), vals(v0, g->d_order);
+  size_t bytes = g->bc_sort_bytes;
+  LUXB_CUDA(cub::DeviceRadixSort::SortPairs(g->d_bc_sort_tmp, bytes, keys, vals, (int)nv, 0, bits, g->stream));
+  if (vals.Current() != g->d_order)
+    LUXB_CUDA(cudaMemcpyAsync(g->d_order, vals.Current(), (size_t)nv * 4, cudaMemcpyDeviceToDevice, g->stream));
+  const uint32_t bound = (uint32_t)std::min<uint64_t>(reached, K);
+  LUXB_TRY(bc_grow(&g->d_bc_off, g->bc_off_cap, (uint64_t)bound + 1));
+  bytes = g->bc_sort_bytes;
+  LUXB_CUDA(cub::DeviceSelect::If(g->d_bc_sort_tmp, bytes, thrust::counting_iterator<uint32_t>(0), g->d_bc_off, ctl + 4, (int)reached,
+                                  BcClassHead{keys.Current()}, g->stream));
+  bc_class_tail_kernel<<<grid_for((uint64_t)bound + 1, 256, grid), 256, 0, g->stream>>>(ctl + 4, bound + 1, reached, g->d_bc_off);
+  LUXB_CUDA(cudaGetLastError());
+  g->bc_off.resize((size_t)bound + 1);
+  LUXB_CUDA(cudaMemcpyAsync(h, ctl + 4, 4, cudaMemcpyDeviceToHost, g->stream));
+  LUXB_CUDA(cudaMemcpyAsync(g->bc_off.data(), g->d_bc_off, ((size_t)bound + 1) * 4, cudaMemcpyDeviceToHost, g->stream));
+  if (g->P > 1) {
+    const uint64_t n = (uint64_t)bound * (g->P + 1);
+    LUXB_TRY(bc_grow(&g->d_bc_split, g->bc_split_cap, n));
+    BcSplitArgs sa{};
+    for (int p = 0; p < g->P; ++p) sa.rl[p] = g->np[p] ? g->rl[p] : nv;
+    sa.rl[g->P] = nv;
+    for (int p = g->P - 1; p >= 0; --p) sa.rl[p] = std::min(sa.rl[p], sa.rl[p + 1]);
+    sa.P = g->P;
+    bc_split_kernel<<<grid_for(n, 256, grid), 256, 0, g->stream>>>(g->d_order, g->d_bc_off, bound, sa, g->d_bc_split);
+    LUXB_CUDA(cudaGetLastError());
+    g->bc_split.resize(n);
+    LUXB_CUDA(cudaMemcpyAsync(g->bc_split.data(), g->d_bc_split, n * 4, cudaMemcpyDeviceToHost, g->stream));
+  }
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  C = h[0];
+  g->bc_off.resize((size_t)C + 1);
+  g->stats.kernel_launches += g->P > 1 ? 6 : 5;
+  return 0;
+}
+
+// one source: BFS levels or weighted distances (the SSSP engine), level / class lists, forward σ, backward δ,
+// scores += δ.  Weighted, "level d" below is distance class d
 static int bc_source(luxb_graph* g, uint32_t s) {
+  const bool weighted = g->cfg.app == LUXB_BC_WEIGHTED;
   g->trace_active.clear();
   g->trace_pull.clear();
   LUXB_TRY(reset_label_state(g, false, s));
   do {
-    LUXB_TRY(label_iteration<HopDistProgram>(g));
+    LUXB_TRY(weighted ? label_iteration<WeightedDistProgram>(g) : label_iteration<HopDistProgram>(g));
     g->stats.iterations++;
   } while (g->stats.last_active != 0);
   uint32_t L = 0;
-  LUXB_TRY(bc_levels(g, L));
+  LUXB_TRY(weighted ? bc_classes(g, L) : bc_levels(g, L));
   const std::vector<uint32_t>& off = g->bc_off;
   uint64_t widest = 0;
   for (uint32_t d = 0; d < L; ++d) widest = std::max<uint64_t>(widest, off[d + 1] - off[d]);
@@ -2637,7 +2720,7 @@ static int bc_source(luxb_graph* g, uint32_t s) {
 int luxb_bc_run(luxb_graph* g, const luxb_vid* sources, int n_sources) {
   LUXB_ARG(g != nullptr, "graph is NULL");
   if (!g->inited) { set_error("luxb_bc_run before luxb_init"); return LUXB_ERR_STATE; }
-  LUXB_ARG(g->cfg.app == LUXB_BC, "luxb_bc_run needs a LUXB_BC handle (this one is app %d)", (int)g->cfg.app);
+  LUXB_ARG(is_bc_app(g->cfg.app), "luxb_bc_run needs a LUXB_BC or LUXB_BC_WEIGHTED handle (this one is app %d)", (int)g->cfg.app);
   LUXB_ARG(n_sources >= 0, "negative source count");
   LUXB_ARG(sources != nullptr || n_sources == 0, "sources is NULL");
   for (int i = 0; i < n_sources; ++i)
@@ -2653,7 +2736,8 @@ int luxb_bc_run(luxb_graph* g, const luxb_vid* sources, int n_sources) {
 int luxb_bc_source_state(luxb_graph* g, uint32_t* lev, double* sigma, double* delta, size_t nv_count) {
   LUXB_ARG(g != nullptr, "graph is NULL");
   if (!g->inited) { set_error("luxb_bc_source_state before luxb_init"); return LUXB_ERR_STATE; }
-  LUXB_ARG(g->cfg.app == LUXB_BC, "luxb_bc_source_state needs a LUXB_BC handle (this one is app %d)", (int)g->cfg.app);
+  LUXB_ARG(is_bc_app(g->cfg.app), "luxb_bc_source_state needs a LUXB_BC or LUXB_BC_WEIGHTED handle (this one is app %d)",
+           (int)g->cfg.app);
   LUXB_ARG(nv_count == g->nv, "nv_count is %zu, the graph has %u vertices", nv_count, g->nv);
   if (!g->bc_has_source) { set_error("luxb_bc_source_state: no source processed yet"); return LUXB_ERR_STATE; }
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
@@ -2666,7 +2750,7 @@ int luxb_bc_source_state(luxb_graph* g, uint32_t* lev, double* sigma, double* de
 
 // the array luxb_get_values / luxb_set_values address: label replica, current values, or betweenness scores
 static void* values_ptr(luxb_graph* g) {
-  if (g->cfg.app == LUXB_BC) return g->d_scores;
+  if (is_bc_app(g->cfg.app)) return g->d_scores;
   return is_label_app(g->cfg.app) ? g->d_val[0] : g->d_val[g->cur];
 }
 
@@ -2746,7 +2830,7 @@ int luxb_set_local_values(luxb_graph* g, const void* host_in, size_t bytes) {
 int luxb_check(luxb_graph* g, uint64_t* mistakes_out) {
   LUXB_ARG(g && mistakes_out, "NULL argument");
   if (!g->inited) { set_error("luxb_check before luxb_init"); return LUXB_ERR_STATE; }
-  LUXB_ARG(g->cfg.app != LUXB_BC, "luxb_check: betweenness centrality has no check; it runs through luxb_bc_run");
+  LUXB_ARG(!is_bc_app(g->cfg.app), "luxb_check: betweenness centrality has no check; it runs through luxb_bc_run");
   LUXB_ARG(is_label_app(g->cfg.app),
            "the reference has no check for pagerank / col_filter (CHECK_TASK_ID is not registered in pull_model.inl:482-521)");
   LUXB_CUDA(cudaSetDevice(g->cfg.device));

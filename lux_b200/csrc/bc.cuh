@@ -8,10 +8,19 @@
 // order and a fixed shuffle tree; a vertex with more than kBcSegment edges is cut into kBcSegment-edge segments whose
 // fp64 partials are added in segment order by bc_combine_kernel.  No floating-point atomics: one rank is bitwise
 // reproducible.  Results land in a level-ordered buffer (position j of the level), which is what the ranks exchange.
+//
+// Weighted betweenness centrality (LUXB_BC_WEIGHTED) runs the same sweeps over distance classes: D[] comes from
+// label_iteration<WeightedDistProgram>, the reached ids are sorted stably by D and class k is one distinct distance.
+// With every weight >= 1 a tight edge (D[u] + w == D[v], 64-bit, D[v] finite) always goes from a smaller class to a
+// larger one, so ascending classes are a topological order of the shortest-path DAG.  The sums are the kernels above
+// with the filter swapped (bc_class_sum_kernel / bc_class_hub_segments_kernel): the vertex's own D replaces the target
+// and the edge's weight is read beside the neighbour id.  Lane order and shuffle tree are the same, so unit weights
+// give the hop-level results bit for bit.
 #pragma once
 #include <stdint.h>
 #include <cuda_runtime.h>
 #include "common.cuh"
+#include "programs.cuh"
 
 namespace luxb {
 
@@ -23,7 +32,7 @@ struct BcHub {
   uint32_t pos;    // position in the level
   uint32_t nseg;   // ceil(deg / kBcSegment)
   uint32_t base;   // its partials: partial[base .. base + nseg)
-  uint32_t pad;
+  uint32_t dist;   // distance classes: D of the vertex (hop levels: 0)
   uint64_t begin;  // first edge
   uint64_t deg;
 };
@@ -52,19 +61,41 @@ struct BcLevelArgs {
   unsigned long long* edges;  // edges scanned
 };
 
+// weighted sums: the CSC weights (σ) or the push CSR's out_w (δ), aligned with nbr
+struct BcClassArgs {
+  BcLevelArgs a;
+  const int32_t* weight;
+};
+
+// a tight edge from -> to: D[from] + w == D[to] without wrap-around, D[to] finite (so a path whose sum saturates to
+// INF never matches, and an unreached tail never does: INF + w > every u32)
+__device__ __forceinline__ bool bc_tight(uint32_t from, int32_t w, uint32_t to) {
+  return to != kDistInf && (uint64_t)from + (uint32_t)w == to;
+}
+
 template <bool kOut>
 __device__ __forceinline__ double bc_term(const BcLevelArgs& a, uint32_t w) {
   if constexpr (kOut) return (1.0 + a.delta[w]) / a.sigma[w];
   else return a.sigma[w];
 }
 
-// sum of f over edges [e0, e1) of one vertex, by one warp; every lane returns the same value
-template <bool kOut>
-__device__ __forceinline__ double bc_warp_sum(const BcLevelArgs& a, uint64_t e0, uint64_t e1, int lane) {
+// sum of f over edges [e0, e1) of one vertex, by one warp; every lane returns the same value.  kW: the edges kept are
+// the tight ones at the vertex's distance dv (weights wt), else the neighbours on level a.target
+template <bool kOut, bool kW>
+__device__ __forceinline__ double bc_warp_sum(const BcLevelArgs& a, const int32_t* wt, uint32_t dv, uint64_t e0, uint64_t e1,
+                                              int lane) {
   double s = 0.0;
   for (uint64_t e = e0 + lane; e < e1; e += 32) {
     const uint32_t w = __ldg(a.nbr + e);
-    if (__ldg(a.lev + w) == a.target) s += bc_term<kOut>(a, w);
+    bool on;
+    if constexpr (kW) {
+      const uint32_t dw = __ldg(a.lev + w);
+      const int32_t wgt = __ldg(wt + e);
+      on = kOut ? bc_tight(dv, wgt, dw) : bc_tight(dw, wgt, dv);
+    } else {
+      on = __ldg(a.lev + w) == a.target;
+    }
+    if (on) s += bc_term<kOut>(a, w);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xFFFFFFFFu, s, o);  // a + b == b + a: the same sum on every lane
@@ -78,18 +109,20 @@ __device__ __forceinline__ void bc_edge_range(const BcLevelArgs& a, uint32_t v, 
   e1 = a.end[r];
 }
 
-template <bool kOut>
-__global__ void __launch_bounds__(kBcThreads) bc_level_sum_kernel(const __grid_constant__ BcLevelArgs a) {
+template <bool kOut, bool kW>
+__device__ __forceinline__ void bc_level_sum(const BcLevelArgs& a, const int32_t* wt) {
   const int lane = threadIdx.x & 31;
   const uint32_t warps = gridDim.x * (kBcThreads / 32);
   unsigned long long scanned = 0;
   for (uint32_t j = blockIdx.x * (kBcThreads / 32) + threadIdx.x / 32; j < a.n; j += warps) {
     uint64_t e0, e1;
-    bc_edge_range<kOut>(a, a.order[j], e0, e1);
+    const uint32_t v = a.order[j];
+    bc_edge_range<kOut>(a, v, e0, e1);
+    const uint32_t dv = kW ? __ldg(a.lev + v) : 0u;
     const uint64_t deg = e1 - e0;
     scanned += deg;
     if (deg <= kBcSegment) {
-      const double s = bc_warp_sum<kOut>(a, e0, e1, lane);
+      const double s = bc_warp_sum<kOut, kW>(a, wt, dv, e0, e1, lane);
       if (lane == 0) a.out[j] = s;
       continue;
     }
@@ -98,18 +131,28 @@ __global__ void __launch_bounds__(kBcThreads) bc_level_sum_kernel(const __grid_c
     if (lane == 0) {
       const uint32_t k = atomicAdd(&a.ctl->n_hub, 1u);
       base = atomicAdd(&a.ctl->n_seg, nseg);
-      a.hubs[k] = BcHub{j, nseg, base, 0u, e0, deg};
+      a.hubs[k] = BcHub{j, nseg, base, dv, e0, deg};
     }
     base = __shfl_sync(0xFFFFFFFFu, base, 0);
-    const double s = bc_warp_sum<kOut>(a, e0, e0 + kBcSegment, lane);
+    const double s = bc_warp_sum<kOut, kW>(a, wt, dv, e0, e0 + kBcSegment, lane);
     if (lane == 0) a.partial[base] = s;
   }
   if (lane == 0 && scanned) atomicAdd(a.edges, scanned);
 }
 
-// segments 1 .. nseg-1 of every hub of the level, spread over all warps of the grid
 template <bool kOut>
-__global__ void __launch_bounds__(kBcThreads) bc_hub_segments_kernel(const __grid_constant__ BcLevelArgs a) {
+__global__ void __launch_bounds__(kBcThreads) bc_level_sum_kernel(const __grid_constant__ BcLevelArgs a) {
+  bc_level_sum<kOut, false>(a, nullptr);
+}
+
+template <bool kOut>
+__global__ void __launch_bounds__(kBcThreads) bc_class_sum_kernel(const __grid_constant__ BcClassArgs c) {
+  bc_level_sum<kOut, true>(c.a, c.weight);
+}
+
+// segments 1 .. nseg-1 of every hub of the level, spread over all warps of the grid
+template <bool kOut, bool kW>
+__device__ __forceinline__ void bc_hub_segments(const BcLevelArgs& a, const int32_t* wt) {
   const int lane = threadIdx.x & 31;
   const uint32_t W = gridDim.x * (kBcThreads / 32);
   const uint32_t gw = blockIdx.x * (kBcThreads / 32) + threadIdx.x / 32;
@@ -122,11 +165,21 @@ __global__ void __launch_bounds__(kBcThreads) bc_hub_segments_kernel(const __gri
       const uint32_t s = k + 1;
       const uint64_t e0 = hub.begin + (uint64_t)s * kBcSegment;
       const uint64_t e1 = min(e0 + kBcSegment, hub.begin + hub.deg);
-      const double sum = bc_warp_sum<kOut>(a, e0, e1, lane);
+      const double sum = bc_warp_sum<kOut, kW>(a, wt, hub.dist, e0, e1, lane);
       if (lane == 0) a.partial[hub.base + s] = sum;
     }
     acc += extra;
   }
+}
+
+template <bool kOut>
+__global__ void __launch_bounds__(kBcThreads) bc_hub_segments_kernel(const __grid_constant__ BcLevelArgs a) {
+  bc_hub_segments<kOut, false>(a, nullptr);
+}
+
+template <bool kOut>
+__global__ void __launch_bounds__(kBcThreads) bc_class_hub_segments_kernel(const __grid_constant__ BcClassArgs c) {
+  bc_hub_segments<kOut, true>(c.a, c.weight);
 }
 
 // each hub's partials in segment order
@@ -169,6 +222,48 @@ __global__ void bc_keys_kernel(const uint32_t* __restrict__ lev, uint32_t nv, ui
 __global__ void bc_level_off_kernel(const uint32_t* __restrict__ key, uint32_t nv, uint32_t* __restrict__ level_off) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += gridDim.x * blockDim.x)
     if (i == 0 || key[i - 1] != key[i]) level_off[key[i]] = i;
+}
+
+// ---- distance classes (weighted) ------------------------------------------------------------------------------------
+// out[0] = largest finite distance, out[1] = number of reached vertices (D != INF: a distance may exceed nv)
+__global__ void bc_dist_max_kernel(const uint32_t* __restrict__ dist, uint32_t nv, uint32_t* __restrict__ out) {
+  uint32_t m = 0, c = 0;
+  for (uint32_t v = blockIdx.x * blockDim.x + threadIdx.x; v < nv; v += gridDim.x * blockDim.x) {
+    const uint32_t d = dist[v];
+    if (d != kDistInf) { m = max(m, d); ++c; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    m = max(m, __shfl_xor_sync(0xFFFFFFFFu, m, o));
+    c += __shfl_xor_sync(0xFFFFFFFFu, c, o);
+  }
+  if ((threadIdx.x & 31) == 0 && c) {
+    atomicMax(out, m);
+    atomicAdd(out + 1, c);
+  }
+}
+
+// sort keys (distance, or K = largest distance + 1 for unreached) and ids
+__global__ void bc_dist_keys_kernel(const uint32_t* __restrict__ dist, uint32_t nv, uint32_t K, uint32_t* __restrict__ key,
+                                    uint32_t* __restrict__ id) {
+  for (uint32_t v = blockIdx.x * blockDim.x + threadIdx.x; v < nv; v += gridDim.x * blockDim.x) {
+    const uint32_t d = dist[v];
+    key[v] = d != kDistInf ? d : K;
+    id[v] = v;
+  }
+}
+
+// position i of the sorted keys starts a class (cub::DeviceSelect::If over the positions gives class_off)
+struct BcClassHead {
+  const uint32_t* key;
+  __device__ __forceinline__ bool operator()(uint32_t i) const { return i == 0 || key[i - 1] != key[i]; }
+};
+
+// class_off[k] = reached for k in [classes, n): entry `classes` closes the last class, and the entries past it (the host
+// reads a bound on the class count, not the count) are empty classes
+__global__ void bc_class_tail_kernel(const uint32_t* __restrict__ classes, uint32_t n, uint32_t reached,
+                                     uint32_t* __restrict__ class_off) {
+  for (uint32_t k = *classes + blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) class_off[k] = reached;
 }
 
 struct BcSplitArgs {

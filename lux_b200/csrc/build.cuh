@@ -234,6 +234,13 @@ __global__ void negative_weight_kernel(const int32_t* __restrict__ w, uint64_t n
   if (c) atomicAdd(bad, c);
 }
 
+// number of weights below `lo` in this rank's slice (weighted betweenness centrality needs w >= 1)
+__global__ void light_weight_kernel(const int32_t* __restrict__ w, uint64_t n, int32_t lo, unsigned long long* __restrict__ bad) {
+  unsigned long long c = 0;
+  for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (uint64_t)gridDim.x * blockDim.x) c += w[e] < lo;
+  if (c) atomicAdd(bad, c);
+}
+
 __global__ void hist_src_kernel(const uint32_t* __restrict__ src, uint64_t n, uint32_t* __restrict__ cnt) {
   for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (uint64_t)gridDim.x * blockDim.x)
     atomicAdd(cnt + src[e], 1u);

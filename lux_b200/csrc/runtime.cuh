@@ -162,16 +162,17 @@ struct luxb_graph {
   double* d_sigma = nullptr;       // [nv] path counts of the last source
   double* d_delta = nullptr;       // [nv] dependencies of the last source
   double* d_scores = nullptr;      // [nv] Σ δ over the sources processed (the handle's values)
-  uint32_t* d_order = nullptr;     // [nv] reached ids sorted stably by level
+  uint32_t* d_order = nullptr;     // [nv] reached ids sorted stably by level (weighted: by distance)
   double* d_bc_lvl = nullptr;      // one level's sums, in level order (grown to the largest level seen)
   uint64_t bc_lvl_cap = 0;
-  uint32_t* d_bc_off = nullptr;    // level_off[L + 1]
+  uint32_t* d_bc_off = nullptr;    // level_off[L + 1] (weighted: class_off, one entry per distinct distance)
   uint64_t bc_off_cap = 0;
   uint32_t* d_bc_split = nullptr;  // nranks > 1: [L][P + 1] every partition's piece of every level
   uint64_t bc_split_cap = 0;
   void* d_bc_sort_tmp = nullptr;
   size_t bc_sort_bytes = 0;
-  uint32_t* d_bc_ctl = nullptr;    // [0..1] BcCtl of the level being summed, [2] deepest level
+  uint32_t* d_bc_ctl = nullptr;    // [0..1] BcCtl of the level being summed, [2] deepest level (weighted: largest
+                                   // distance), [3] weighted: reached vertices, [4] weighted: class count
   luxb::BcHub* d_bc_hubs = nullptr;
   double* d_bc_partial = nullptr;
   std::vector<uint32_t> bc_off, bc_split;  // host copies of this source's level_off / split

@@ -10,6 +10,7 @@ kernel takes part in the computation, and there is no CPU fallback (the ops rais
     x      = torch.ops.luxb.colfilter(row_end, src, weight, 10) # f32 [nv, 20]
     dist   = torch.ops.luxb.sssp_weighted(row_end, src, weight, 0)  # i64 [nv]  (weighted distance, INF = 2^32 - 1)
     bc     = torch.ops.luxb.betweenness(row_end, src, sources)  # f64 [nv]  (Σ over sources of Brandes' δ, not normalised)
+    bc     = torch.ops.luxb.betweenness_weighted(row_end, src, weight, sources)  # f64 [nv]  (weighted paths, weights >= 1)
 row_end: int64 [nv] END offsets (the .lux convention); src: int64/int32 [ne]; weight: int32 [ne]; sources: int64/int32 [k] vertex ids."""
 import numpy as np
 import torch
@@ -32,6 +33,7 @@ _lib.define("sssp(Tensor row_end, Tensor src, int start) -> Tensor")
 _lib.define("colfilter(Tensor row_end, Tensor src, Tensor weight, int num_iter) -> Tensor")
 _lib.define("sssp_weighted(Tensor row_end, Tensor src, Tensor weight, int start) -> Tensor")
 _lib.define("betweenness(Tensor row_end, Tensor src, Tensor sources) -> Tensor")
+_lib.define("betweenness_weighted(Tensor row_end, Tensor src, Tensor weight, Tensor sources) -> Tensor")
 
 
 def _pagerank(row_end, src, num_iter):
@@ -66,6 +68,12 @@ def _betweenness(row_end, src, sources):
     return torch.from_numpy(out).to(row_end.device)
 
 
+def _betweenness_weighted(row_end, src, weight, sources):
+    out = _apps.betweenness(_np(row_end, np.uint64), _np(src, np.uint32), sources=_np(sources, np.int64), device=_device_index(row_end),
+                            weight=_np(weight, np.int32))
+    return torch.from_numpy(out).to(row_end.device)
+
+
 for _name, _fn in (("pagerank", _pagerank), ("components", _components), ("sssp", _sssp), ("colfilter", _colfilter),
-                   ("sssp_weighted", _sssp_weighted), ("betweenness", _betweenness)):
+                   ("sssp_weighted", _sssp_weighted), ("betweenness", _betweenness), ("betweenness_weighted", _betweenness_weighted)):
     _lib.impl(_name, _fn, "CompositeExplicitAutograd")

@@ -8,7 +8,12 @@ and K - 1 seeded vertices with out-degree > 0 (numpy.random.default_rng(--seed) 
   a parity flag against the CPU oracle (tests/bc_oracle.c) with its CPU time and core count; and, in the same call,
   unweighted SSSP from vertex 0 (scripts/bench_sssp.py's BFS) for the BFS part.
 
-  python scripts/bench_bc.py [--gpus N] [--scale 24] [--k 8] [--reps 3] [--seed 1] [--no-oracle]
+  python scripts/bench_bc.py [--gpus N] [--scale 24] [--k 8] [--reps 3] [--seed 1] [--no-oracle] [--weighted]
+
+--weighted runs weighted BC instead, over the generator's [1, 255] weights (luxb_open_rmat), with the same sources: the
+SSSP part is then weighted SSSP, "levels" are distance classes (from the weighted oracle, tests/bc_weighted_oracle.c,
+which also gives the parity flag) and the reference SSSP run is weighted SSSP from vertex 0.  Both modes report the
+kernel launches per source (luxb_stats kernel_launches), which bound the per-level / per-class overhead.
 
 Algorithmic bound: each of the sigma and delta sweeps reads an id and a level per reached edge, 8 bytes, so
 8 * ne bytes per sweep at most; the JSON line states each sweep's time against that volume at the data-sheet 3.35 TB/s."""
@@ -66,6 +71,7 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--seed", type=int, default=1)
     ap.add_argument("--no-oracle", action="store_true")
+    ap.add_argument("--weighted", action="store_true")
     args = ap.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if args.gpus > 1 and world == 1:
@@ -82,7 +88,8 @@ def main():
     scale, seed = args.scale, 24
     nv, ne = 1 << scale, 16 << scale
     name, power = card()
-    result = dict(bench="bc", graph="RMAT-%d ef16 seed %d" % (scale, seed), nv=nv, ne=ne, gpus=world, card=name, power_limit=power,
+    bc_app, sssp_app = (L.APP_BC_WEIGHTED, L.APP_SSSP_WEIGHTED) if args.weighted else (L.APP_BC, L.APP_SSSP)
+    result = dict(bench="bc_weighted" if args.weighted else "bc", graph="RMAT-%d ef16 seed %d" % (scale, seed), nv=nv, ne=ne, gpus=world, card=name, power_limit=power,
                   k=args.k)
     exchange = L.EXCHANGE_P2P if world > 1 else L.EXCHANGE_NCCL
 
@@ -103,17 +110,17 @@ def main():
         dist.all_reduce(v[1:], op=dist.ReduceOp.SUM)
         return float(tmax), int(v[1])
 
-    # the BFS alone: unweighted SSSP from vertex 0
+    # the BFS (weighted: the weighted SSSP) alone, from vertex 0
     sssp_t = []
     for _ in range(max(args.reps, 1)):
-        g = open_graph(L.APP_SSSP)
+        g = open_graph(sssp_app)
         it = g.run_to_convergence()
         sssp_t.append(reduce_max_sum(g.stats()["loop_seconds"], 0)[0])
         g.close()
     result["sssp_from_0"] = dict(iterations=it, ms_median=1e3 * float(np.median(sssp_t)), ms_min=1e3 * min(sssp_t))
 
-    g = open_graph(L.APP_BC)
-    row_end, src = g.local_csc()
+    g = open_graph(bc_app)
+    row_end, src, weight = g.local_csc(weighted=True) if args.weighted else (g.local_csc() + (None,))
     outdeg = np.bincount(src, minlength=nv).astype(np.int64)
     if world > 1:
         t = torch.from_numpy(outdeg).cuda()
@@ -126,6 +133,7 @@ def main():
     os.environ["LUXB_PHASE_TIMING"] = "2"  # one line of phase means per luxb_bc_run call
     per_source = {"total": [], "sigma": [], "delta": []}
     edges = 0
+    k0 = g.stats()["kernel_launches"]
     for rep in range(max(args.reps, 1)):
         e0 = g.stats()["edges_processed"]
         t0 = g.stats()["loop_seconds"]
@@ -143,6 +151,7 @@ def main():
         per_source["delta"].append(dl / len(sources))
         edges = e
     os.environ.pop("LUXB_PHASE_TIMING")
+    launches = (g.stats()["kernel_launches"] - k0) / (len(sources) * max(args.reps, 1))
     bc = g.values()
     g.close()
     med = {k: float(np.median(v)) for k, v in per_source.items()}
@@ -150,18 +159,26 @@ def main():
     result["ms_per_source"] = dict(median=med["total"], min=min(per_source["total"]), sigma_median=med["sigma"], delta_median=med["delta"],
                                    bfs_and_levels_median=med["total"] - med["sigma"] - med["delta"], reps=len(per_source["total"]))
     result["edges_touched_per_run"] = edges
+    result["kernel_launches_per_source"] = launches
     result["mteps"] = ne * len(sources) / (med["total"] * 1e-3 * len(sources)) / 1e6
     result["sweep_bound_ms_at_datasheet"] = bound_ms
     result["sigma_fraction_of_datasheet"] = bound_ms / med["sigma"] if med["sigma"] else None
     result["delta_fraction_of_datasheet"] = bound_ms / med["delta"] if med["delta"] else None
     if rank == 0 and not args.no_oracle:
         import bc_oracle as B
+        import bc_weighted_oracle as BW
+        import weighted_oracle as WO
         import oracle as O
         if world > 1:
             row_end, src = O.gen_rmat_csc(scale, nv, ne, seed)
+            weight = WO.rmat_weights(seed, row_end, src) if args.weighted else None
         t0 = time.perf_counter()
-        ref = B.run(row_end, src, sources)
-        result["levels_per_source"] = ref["levels"].tolist()
+        if args.weighted:
+            ref = BW.run(row_end, src, weight, sources)
+            result["classes_per_source"] = ref["classes"].tolist()
+        else:
+            ref = B.run(row_end, src, sources)
+            result["levels_per_source"] = ref["levels"].tolist()
         result["oracle_cpu_s"] = time.perf_counter() - t0
         reps = max(args.reps, 1)
         want = ref["scores"] * reps  # every rep added the same K sources
