@@ -9,6 +9,7 @@
                                                                                    # betweenness centrality (ours)
   python apps/lux_cli.py bc         -weighted -file w.lux [-start v | -nsrc K -seed S] [-out scores.npy]
                                                                                    # weighted BC (i32 trailer, w >= 1; ours)
+  python apps/lux_cli.py tc         -ng 1 -file g.lux [-out t.npy]                  # triangle counting (ours)
   python apps/lux_cli.py converter  -nv N -ne M -input edges.txt -output g.lux     # tools/converter.cc:13-39 (host only)
 
 `-ll:gpu N` is accepted as a synonym of `-ng N` (README.md:47); -ll:fsize / -ll:zsize are accepted and ignored (HBM is
@@ -23,6 +24,10 @@ numpy.random.default_rng(S).choice(nv, K, replace=False) with `-seed S` (default
 (exact BC).  It prints "ELAPSED TIME" (device time of the BC run) and no "[Memory Setting]" line: the reference has no
 formula for BC.  `bc -weighted` reads the .lux i32 weight trailer and runs weighted BC (shortest paths by weighted
 distance, every weight >= 1) with the same source flags.
+
+`tc` (no reference counterpart) counts the triangles of the graph read as undirected and simple (self-loops, parallel
+edges and both directions of an edge collapse; weights are ignored).  It prints "ELAPSED TIME" (device time of the count)
+and "TRIANGLES = T" on rank 0, and no "[Memory Setting]" line; `-out` saves the u64 triangle count of every vertex.
 """
 import os
 import subprocess
@@ -33,7 +38,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-APPS = {"pagerank": 0, "components": 1, "sssp": 2, "colfilter": 3, "bc": 5}
+APPS = {"pagerank": 0, "components": 1, "sssp": 2, "colfilter": 3, "bc": 5, "tc": 7}
 
 
 def parse(argv):
@@ -155,7 +160,7 @@ def main():
     g = L.LuxGraph.from_file(opt["file"], app=weighted_app[app] if weighted else APPS[app], rank=rank, nranks=world, device=local,
                              start=opt["start"], verbose=opt["verbose"])
     b = g.bounds()
-    if rank == 0 and app != "bc":
+    if rank == 0 and app not in ("bc", "tc"):
         fb, zc = memory_setting(app, g.nv, g.ne, b, int(b["fq_right"][-1]) + 1, weighted)
         print("[Memory Setting] Set ll:fsize >= %dMB and ll:zsize >= %dMB" % (fb, zc), flush=True)
     g.comm_init_torch()
@@ -164,10 +169,14 @@ def main():
         g.iterate(opt["ni"])
     elif app == "bc":
         g.bc_run(bc_sources(opt, g.nv))
+    elif app == "tc":
+        total = g.tc_run()
     else:
         g.run_to_convergence()
     if rank == 0:
         print("ELAPSED TIME = %7.7f s" % g.stats()["loop_seconds"], flush=True)
+        if app == "tc":
+            print("TRIANGLES = %d" % total, flush=True)
     if opt["check"] and app in ("components", "sssp"):
         bad = g.check()
         print("[%s] Check task: rowLeft(%u) numMistakes(%u)" % ("PASS" if bad == 0 else "FAIL", int(b["row_left"][rank]), bad),

@@ -52,8 +52,10 @@ typedef enum {
   LUXB_SSSP_WEIGHTED = 4, /* weighted SSSP (no reference counterpart) — push/pull hybrid, u32 distance, INF = LUXB_DIST_INF */
   LUXB_BC = 5,           /* betweenness centrality (no reference counterpart) — Brandes over the SSSP engine's hop levels,
                             f64 score per vertex; runs through luxb_bc_run */
-  LUXB_BC_WEIGHTED = 6   /* weighted betweenness centrality (no reference counterpart) — Brandes over the weighted SSSP
+  LUXB_BC_WEIGHTED = 6,  /* weighted betweenness centrality (no reference counterpart) — Brandes over the weighted SSSP
                             distances (weights >= 1), f64 score per vertex; runs through luxb_bc_run */
+  LUXB_TC = 7            /* triangle counting (no reference counterpart) — exact u64 count of the triangles at every
+                            vertex of the undirected simple graph; runs through luxb_tc_run */
 } luxb_app;
 
 /* Weighted SSSP (LUXB_SSSP_WEIGHTED):
@@ -103,6 +105,21 @@ typedef enum {
  * LUXB_BC exactly: D = lev, and sigma, delta and the scores are bit for bit equal.  luxb_bc_source_state returns D as
  * `lev`.  Values, luxb_iterate / luxb_run_to_convergence / luxb_check, luxb_stats and the phase timing behave as for
  * LUXB_BC; luxb_trace holds the weighted SSSP trace of the last source. */
+
+/* Triangle counting (LUXB_TC).  The CSC's directed edges are read as an undirected simple graph: {u, v} is an edge iff
+ * u != v and at least one of u -> v or v -> u is stored.  Parallel edges, both directions and self-loops collapse to that
+ * one edge; weights are ignored (a weighted CSC is accepted).  A triangle is a set of three distinct, pairwise adjacent
+ * vertices.
+ *  - t[v] is the number of triangles that contain v, u64 (networkx's triangles() on the simple graph);
+ *  - the total T = sum of t / 3, u64;
+ *  - integers only: the results depend neither on the schedule nor on the number of ranks or the split.
+ * luxb_init builds the oriented adjacency once (every rank holds the whole graph: its slice's edges are exchanged at
+ * luxb_init); luxb_open_* read the input edges once, as for every app.  The handle's values (luxb_get_values /
+ * luxb_get_local_values) are t, 8 bytes per vertex: zeros before the first luxb_tc_run, complete on every rank after one
+ * (the get calls are not collective).  luxb_set_values / luxb_set_local_values, luxb_iterate, luxb_run_to_convergence and
+ * luxb_check return LUXB_ERR_ARG.  luxb_stats: iterations = luxb_tc_run calls, edges_processed += m (undirected simple
+ * edges) per call, loop_seconds = device time of the luxb_tc_run calls.  luxb_get_local_csc / luxb_device_view keep
+ * returning this rank's CSC slice.  cfg.start_vtx, cfg.exchange and cfg.verbose have no effect. */
 
 typedef enum {
   LUXB_EXCHANGE_NCCL = 0, /* library collectives only: PageRank packs its share and broadcasts the two ranges of every
@@ -218,7 +235,7 @@ int luxb_iterate(luxb_graph* g, int iters, uint64_t* active_out);
 int luxb_run_to_convergence(luxb_graph* g, int max_iters, int* iters_out);
 
 /* ---- results / check / stats -------------------------------------------------------------------------------- */
-/* Full vertex-value array (what the reference holds in dist_lr[iter%2]): nv * {4 | 4 | 80 | 8 (BC scores)} bytes.  PageRank on
+/* Full vertex-value array (what the reference holds in dist_lr[iter%2]): nv * {4 | 4 | 80 | 8 (BC scores, TC counts)} bytes.  PageRank on
  * nranks > 1 exchanges only the values that are ever gathered each iteration and completes the full array on demand:
  * there the call is collective (every rank calls it at the same point). */
 int luxb_get_values(luxb_graph* g, void* host_out, size_t bytes);
@@ -290,6 +307,12 @@ int luxb_bc_run(luxb_graph* g, const luxb_vid* sources, int n_sources);
 /* The full lev / sigma / delta arrays (nv_count == nv entries each) of the last source processed (LUXB_BC_WEIGHTED: lev
  * is the u32 distance D); a NULL pointer skips that array.  Every rank holds them complete: not collective.  LUXB_ERR_STATE before the first source. */
 int luxb_bc_source_state(luxb_graph* g, uint32_t* lev, double* sigma, double* delta, size_t nv_count);
+
+/* ---- triangle counting (LUXB_TC handles) --------------------------------------------------------------------------- */
+/* Recount t from zero and write the total T to *total_out (may be NULL).  Every call gives the same result.  Collective on
+ * nranks > 1: each rank counts the triangles found at the vertices of its own range, then t is summed over the ranks.
+ * LUXB_ERR_STATE before luxb_init, LUXB_ERR_ARG on another app. */
+int luxb_tc_run(luxb_graph* g, uint64_t* total_out);
 
 void luxb_close(luxb_graph* g);
 const char* luxb_last_error(void);

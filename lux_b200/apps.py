@@ -6,11 +6,12 @@ sssp       : sssp/sssp.cc                     (same loop, -start; with weights: 
 colfilter  : col_filter/colfilter.cc:71-81    (-ni fixed iterations)
 betweenness: Brandes from a list of sources over the SSSP engine's hop levels, or with weights over the weighted
              SSSP distances (ours; the reference has no BC)
+triangles  : exact triangle counts of the undirected simple graph (ours)
 Single-rank convenience wrappers; multi-GPU callers drive LuxGraph directly (see bench.py).
 """
 import numpy as np
 
-from .binding import LuxGraph, APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC, APP_BC_WEIGHTED
+from .binding import LuxGraph, APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC, APP_BC_WEIGHTED, APP_TC
 
 
 def pagerank(row_end, src, num_iter=10, device=0):
@@ -63,3 +64,13 @@ def betweenness(row_end, src, sources=None, device=0, weight=None):
         g.init()
         g.bc_run(srcs)
         return g.values()
+
+
+def triangles(row_end, src, device=0):
+    """Triangle counts of the CSC read as an undirected simple graph ({u, v} is an edge iff u != v and u -> v or v -> u is
+    stored; weights are ignored): dict(total = number of triangles, per_vertex = u64 [nv] triangles containing each
+    vertex)."""
+    with LuxGraph.from_csc(row_end, src, app=APP_TC, device=device) as g:
+        g.init()
+        total = g.tc_run()
+        return dict(total=total, per_vertex=g.values())

@@ -6,7 +6,7 @@ import numpy as np
 
 from . import build as _build
 
-APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC, APP_BC_WEIGHTED = 0, 1, 2, 3, 4, 5, 6
+APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC, APP_BC_WEIGHTED, APP_TC = 0, 1, 2, 3, 4, 5, 6, 7
 DIST_INF = 0xFFFFFFFF  # APP_SSSP_WEIGHTED / APP_BC_WEIGHTED: distance of an unreachable vertex (LUXB_DIST_INF)
 EXCHANGE_NCCL, EXCHANGE_P2P, EXCHANGE_P2P_FUSED = 0, 1, 2
 DENSE_BITMAP, SPARSE_QUEUE = 0x1234567, 0x7654321
@@ -120,7 +120,8 @@ def convert_edgelist(edge_list_path, lux_path, nv, ne):
 
 
 _VDTYPE = {APP_PAGERANK: np.float32, APP_CC: np.uint32, APP_SSSP: np.uint32, APP_COLFILTER: np.float32,
-           APP_SSSP_WEIGHTED: np.uint32, APP_BC: np.float64, APP_BC_WEIGHTED: np.float64}
+           APP_SSSP_WEIGHTED: np.uint32, APP_BC: np.float64, APP_BC_WEIGHTED: np.float64,
+           APP_TC: np.uint64}
 
 
 class LuxGraph:
@@ -327,6 +328,13 @@ class LuxGraph:
         _chk(load_library().luxb_bc_source_state(self._h, _p(lev), _p(sigma), _p(delta), C.c_size_t(self.nv)),
              "luxb_bc_source_state")
         return lev, sigma, delta
+
+    def tc_run(self):
+        """Triangle counting (APP_TC handles): recount the triangles at every vertex of the undirected simple graph (the
+        u64 values() returns) and return the total.  Collective on nranks > 1."""
+        total = C.c_uint64(0)
+        _chk(load_library().luxb_tc_run(self._h, C.byref(total)), "luxb_tc_run")
+        return total.value
 
     def enable_kernel_timing(self, on=True):
         _chk(load_library().luxb_enable_kernel_timing(self._h, C.c_int(1 if on else 0)), "luxb_enable_kernel_timing")

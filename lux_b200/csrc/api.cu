@@ -21,6 +21,8 @@
 using namespace luxb;
 // betweenness centrality, over hop levels or over weighted distance classes: luxb_bc_run instead of luxb_iterate
 static bool is_bc_app(luxb_app app) { return app == LUXB_BC || app == LUXB_BC_WEIGHTED; }
+// triangle counting: luxb_tc_run instead of luxb_iterate, u64 counts as values
+static bool is_tc_app(luxb_app app) { return app == LUXB_TC; }
 // labels are weighted distances (u32, INF = LUXB_DIST_INF, label_iteration<WeightedDistProgram>): the app reads the CSC
 // weights, keeps out_w beside the push CSR and pulls through the merge-path sweep only
 static bool weighted_labels(luxb_app app) { return app == LUXB_SSSP_WEIGHTED || app == LUXB_BC_WEIGHTED; }
@@ -245,7 +247,7 @@ static bool use_balanced_split(const luxb_config* cfg) {
 
 static int check_config(const luxb_config* cfg) {
   LUXB_ARG(cfg != nullptr, "config is NULL");
-  LUXB_ARG(cfg->app >= LUXB_PAGERANK && cfg->app <= LUXB_BC_WEIGHTED, "unknown app %d", (int)cfg->app);
+  LUXB_ARG(cfg->app >= LUXB_PAGERANK && cfg->app <= LUXB_TC, "unknown app %d", (int)cfg->app);
   LUXB_ARG(cfg->nranks >= 1 && cfg->nranks <= LUXB_MAX_PARTS, "nranks %d out of range [1,%d]", cfg->nranks, LUXB_MAX_PARTS);
   LUXB_ARG(cfg->rank >= 0 && cfg->rank < cfg->nranks, "rank %d out of range", cfg->rank);
   return 0;
@@ -1121,6 +1123,7 @@ static int build_seg_sweep(luxb_graph* g);
 static int pagerank_publish(luxb_graph* g, float* x_new);
 static int wait_cold_exchange(luxb_graph* g);
 static int bc_alloc(luxb_graph* g);
+static int tc_build(luxb_graph* g);
 
 // The gather side of the pull sweeps: global out-degrees, the hot set (build_hot_layout), the flagged streams if
 // `streams` (build_seg_sweep) and the hot copies Z = [hot | compact cold values on one rank] + one whole table of slack:
@@ -1225,6 +1228,11 @@ int luxb_init(luxb_graph* g) {
         LUXB_CUDA(cudaStreamSynchronize(g->stream));
       }
       if (is_bc_app(g->cfg.app)) LUXB_TRY(bc_alloc(g));
+      break;
+    }
+    case LUXB_TC: {
+      g->vbytes = 8;
+      LUXB_TRY(tc_build(g));
       break;
     }
   }
@@ -2445,6 +2453,7 @@ int luxb_iterate(luxb_graph* g, int iters, uint64_t* active_out) {
   LUXB_ARG(g != nullptr, "graph is NULL");
   if (!g->inited) { set_error("luxb_iterate before luxb_init"); return LUXB_ERR_STATE; }
   LUXB_ARG(!is_bc_app(g->cfg.app), "luxb_iterate: betweenness centrality runs through luxb_bc_run");
+  LUXB_ARG(!is_tc_app(g->cfg.app), "luxb_iterate: triangle counting runs through luxb_tc_run");
   LUXB_ARG(iters >= 0, "negative iteration count");
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
   if (const char* env = getenv("LUXB_PHASE_TIMING")) { g->pt.on = atoi(env) != 0; g->pt.per_call = atoi(env) == 2; }  // may change between calls
@@ -2462,6 +2471,7 @@ int luxb_run_to_convergence(luxb_graph* g, int max_iters, int* iters_out) {
   LUXB_ARG(g != nullptr, "graph is NULL");
   if (!g->inited) { set_error("luxb_run_to_convergence before luxb_init"); return LUXB_ERR_STATE; }
   LUXB_ARG(!is_bc_app(g->cfg.app), "luxb_run_to_convergence: betweenness centrality runs through luxb_bc_run");
+  LUXB_ARG(!is_tc_app(g->cfg.app), "luxb_run_to_convergence: triangle counting runs through luxb_tc_run");
   LUXB_ARG(is_label_app(g->cfg.app), "only push apps converge (pagerank/col_filter run -ni iterations)");
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
   LUXB_CUDA(cudaEventRecord(g->ev_begin, g->stream));
@@ -2748,9 +2758,206 @@ int luxb_bc_source_state(luxb_graph* g, uint32_t* lev, double* sigma, double* de
   return 0;
 }
 
+// ---- triangle counting (tc.cuh) ------------------------------------------------------------------------------------
+// sort keys[0, n) over their low `bits` bits and keep the distinct ones, at the front of keys; *m = their number
+static int tc_sort_unique(luxb_graph* g, DevTmp& tmp, uint64_t* keys, uint64_t* alt, uint64_t n, int bits, uint64_t* m) {
+  *m = 0;
+  if (n == 0) return 0;
+  cub::DoubleBuffer<uint64_t> db(keys, alt);
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortKeys(t, b, db, (long long)n, 0, bits, g->stream);
+  }));
+  unsigned long long* d_n = nullptr;
+  LUXB_TRY(tmp.alloc(&d_n, 1));
+  uint64_t* out = db.Current() == keys ? alt : keys;
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceSelect::Unique(t, b, db.Current(), out, d_n, (long long)n, g->stream);
+  }));
+  unsigned long long cnt = 0;
+  LUXB_CUDA(cudaMemcpyAsync(&cnt, d_n, 8, cudaMemcpyDeviceToHost, g->stream));
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  tmp.release(d_n);
+  if (out != keys) LUXB_CUDA(cudaMemcpyAsync(keys, out, cnt * 8, cudaMemcpyDeviceToDevice, g->stream));
+  *m = cnt;
+  return 0;
+}
+
+// luxb_init of a LUXB_TC handle: the undirected simple edges of the whole graph (on several ranks every rank's distinct
+// keys go to every rank), the oriented out-lists, the work per vertex and the bins of this rank's range
+static int tc_build(luxb_graph* g) {
+  DevTmp tmp;
+  const int grid = g->num_sms * 8;
+  const uint32_t nv = g->nv;
+  int vbits = 1;
+  while ((1ull << vbits) < (uint64_t)nv) ++vbits;
+  const int bits = 32 + vbits;  // min < nv in the high word, max in the low one
+  uint64_t *d_keys = nullptr, *d_alt = nullptr;
+  unsigned long long* d_cur = nullptr;
+  LUXB_TRY(tmp.alloc(&d_keys, g->e_part));
+  LUXB_TRY(tmp.alloc(&d_alt, g->e_part));
+  LUXB_TRY(tmp.alloc(&d_cur, 1));
+  LUXB_CUDA(cudaMemsetAsync(d_cur, 0, 8, g->stream));
+  if (g->e_part)
+    tc_emit_keys_kernel<<<grid_for(g->e_part, 256, grid), 256, 0, g->stream>>>(g->d_row_end, g->n_part, g->e_part, g->row_left, g->d_src,
+                                                                             d_cur, d_keys);
+  LUXB_CUDA(cudaGetLastError());
+  unsigned long long n_keys = 0;
+  LUXB_CUDA(cudaMemcpyAsync(&n_keys, d_cur, 8, cudaMemcpyDeviceToHost, g->stream));
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  uint64_t m = 0;
+  LUXB_TRY(tc_sort_unique(g, tmp, d_keys, d_alt, n_keys, bits, &m));
+  if (g->P > 1) {  // every rank's distinct keys to every rank (one grouped set of broadcasts), distinct again
+    uint64_t* d_counts = nullptr;
+    LUXB_TRY(tmp.alloc(&d_counts, (uint64_t)g->P + 1));
+    LUXB_CUDA(cudaMemcpyAsync(d_counts + g->P, &m, 8, cudaMemcpyHostToDevice, g->stream));
+    LUXB_NCCL(nccl().AllGather(d_counts + g->P, d_counts, 1, ncclUint64, g->comm, g->stream));
+    std::vector<uint64_t> counts(g->P);
+    LUXB_CUDA(cudaMemcpyAsync(counts.data(), d_counts, (size_t)g->P * 8, cudaMemcpyDeviceToHost, g->stream));
+    LUXB_CUDA(cudaStreamSynchronize(g->stream));
+    uint64_t total = 0;
+    for (uint64_t c : counts) total += c;
+    uint64_t *d_all = nullptr, *d_all_alt = nullptr;
+    LUXB_TRY(tmp.alloc(&d_all, total));
+    LUXB_TRY(tmp.alloc(&d_all_alt, total));
+    LUXB_NCCL(nccl().GroupStart());
+    uint64_t at = 0;
+    for (int p = 0; p < g->P; ++p) {
+      if (counts[p]) LUXB_NCCL(nccl().Broadcast(p == g->cfg.rank ? d_keys : d_all + at, d_all + at, counts[p], ncclUint64, p, g->comm, g->stream));
+      at += counts[p];
+    }
+    LUXB_NCCL(nccl().GroupEnd());
+    LUXB_CUDA(cudaStreamSynchronize(g->stream));
+    tmp.release(d_keys);
+    tmp.release(d_alt);
+    d_keys = d_all;
+    d_alt = d_all_alt;
+    LUXB_TRY(tc_sort_unique(g, tmp, d_keys, d_alt, total, bits, &m));
+  }
+  g->tc_m = m;
+  // degrees, orientation, out-lists sorted by (from, to), offsets and the work W(u)
+  uint32_t *d_deg = nullptr, *d_outdeg = nullptr;
+  unsigned long long* d_work = nullptr;
+  LUXB_TRY(tmp.alloc(&d_deg, nv));
+  LUXB_TRY(tmp.alloc(&d_outdeg, nv));
+  LUXB_TRY(tmp.alloc(&d_work, nv));
+  LUXB_CUDA(cudaMemsetAsync(d_deg, 0, (size_t)nv * 4, g->stream));
+  LUXB_CUDA(cudaMemsetAsync(d_outdeg, 0, (size_t)nv * 4, g->stream));
+  LUXB_CUDA(cudaMemsetAsync(d_work, 0, (size_t)nv * 8, g->stream));
+  const uint64_t* d_sorted = d_keys;
+  if (m) {
+    tc_degree_kernel<<<grid_for(m, 256, grid), 256, 0, g->stream>>>(d_keys, m, d_deg);
+    tc_orient_kernel<<<grid_for(m, 256, grid), 256, 0, g->stream>>>(d_keys, m, d_deg, d_outdeg);
+    LUXB_CUDA(cudaGetLastError());
+    cub::DoubleBuffer<uint64_t> db(d_keys, d_alt);
+    LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+      return cub::DeviceRadixSort::SortKeys(t, b, db, (long long)m, 0, bits, g->stream);
+    }));
+    d_sorted = db.Current();
+  }
+  LUXB_TRY(dmalloc(&g->d_tc_off, (uint64_t)nv + 1));
+  LUXB_CUDA(cudaMemsetAsync(g->d_tc_off + nv, 0, 8, g->stream));
+  widen_u32_to_u64_kernel<<<grid_for(nv, 256, grid), 256, 0, g->stream>>>(d_outdeg, g->d_tc_off, nv);
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceScan::ExclusiveSum(t, b, g->d_tc_off, g->d_tc_off, (long long)nv + 1, g->stream);
+  }));
+  LUXB_TRY(dmalloc(&g->d_tc_dst, m + 8));
+  if (m) tc_lists_kernel<<<grid_for(m, 256, grid), 256, 0, g->stream>>>(d_sorted, m, g->d_tc_off, g->d_tc_dst, d_work);
+  LUXB_CUDA(cudaGetLastError());
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  for (void* q : {(void*)d_keys, (void*)d_alt, (void*)d_deg, (void*)d_outdeg}) tmp.release(q);
+  // bins of this rank's range: staged vertices (grouped kernel) and big ones
+  uint32_t* d_sel = nullptr;
+  LUXB_TRY(tmp.alloc(&d_sel, 2));
+  LUXB_TRY(dmalloc(&g->d_tc_staged, g->n_part));
+  LUXB_TRY(dmalloc(&g->d_tc_big, g->n_part));
+  uint32_t n_sel[2] = {0, 0};
+  if (g->n_part) {
+    thrust::counting_iterator<uint32_t> ids(g->row_left);
+    LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+      return cub::DeviceSelect::If(t, b, ids, g->d_tc_staged, d_sel, (int)g->n_part, TcStaged{g->d_tc_off}, g->stream);
+    }));
+    LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+      return cub::DeviceSelect::If(t, b, ids, g->d_tc_big, d_sel + 1, (int)g->n_part, TcBig{g->d_tc_off}, g->stream);
+    }));
+    LUXB_CUDA(cudaMemcpyAsync(n_sel, d_sel, 8, cudaMemcpyDeviceToHost, g->stream));
+    LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  }
+  const uint32_t n_staged = n_sel[0];
+  g->tc_n_big = n_sel[1];
+  // groups: exclusive prefixes of the staged list lengths and costs, a head wherever either crosses its multiple
+  uint64_t* d_cost = nullptr;
+  LUXB_TRY(tmp.alloc(&d_cost, (uint64_t)n_staged + 1));
+  LUXB_TRY(dmalloc(&g->d_tc_stage_pre, (uint64_t)n_staged + 1));
+  tc_cost_kernel<<<grid_for((uint64_t)n_staged + 1, 256, grid), 256, 0, g->stream>>>(g->d_tc_staged, n_staged, g->d_tc_off, d_work,
+                                                                                    g->d_tc_stage_pre, d_cost);
+  LUXB_CUDA(cudaGetLastError());
+  for (uint64_t* p : {g->d_tc_stage_pre, d_cost})
+    LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+      return cub::DeviceScan::ExclusiveSum(t, b, p, p, (long long)n_staged + 1, g->stream);
+    }));
+  LUXB_TRY(dmalloc(&g->d_tc_group, (uint64_t)n_staged + 1));
+  uint32_t n_group = 0;
+  if (n_staged) {
+    LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+      return cub::DeviceSelect::If(t, b, thrust::counting_iterator<uint32_t>(0), g->d_tc_group, d_sel, (int)n_staged,
+                                   TcGroupHead{g->d_tc_stage_pre, d_cost}, g->stream);
+    }));
+    LUXB_CUDA(cudaMemcpyAsync(&n_group, d_sel, 4, cudaMemcpyDeviceToHost, g->stream));
+    LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  }
+  LUXB_CUDA(cudaMemcpyAsync(g->d_tc_group + n_group, &n_staged, 4, cudaMemcpyHostToDevice, g->stream));
+  g->tc_n_group = n_group;
+  // the run's state: t, its sum, the work counters; a grid of resident CTAs per kernel
+  LUXB_TRY(dmalloc(&g->d_tc_t, nv));
+  LUXB_CUDA(cudaMemsetAsync(g->d_tc_t, 0, (size_t)nv * 8, g->stream));
+  LUXB_TRY(dmalloc(&g->d_tc_total, 1));
+  LUXB_TRY(dmalloc(&g->d_tc_next, 2));
+  LUXB_CUDA(cub::DeviceReduce::Sum(nullptr, g->tc_sum_bytes, g->d_tc_t, g->d_tc_total, (long long)nv, g->stream));
+  LUXB_TRY(dmalloc((char**)&g->d_tc_sum_tmp, g->tc_sum_bytes));
+  int per_sm = 0;
+  LUXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, tc_group_kernel, kTcThreads, 0));
+  g->tc_group_grid = std::max(per_sm, 1) * g->num_sms;
+  LUXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, tc_big_kernel, kTcThreads, 0));
+  g->tc_big_grid = std::max(per_sm, 1) * g->num_sms;
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  return 0;
+}
+
+int luxb_tc_run(luxb_graph* g, uint64_t* total_out) {
+  LUXB_ARG(g != nullptr, "graph is NULL");
+  if (!g->inited) { set_error("luxb_tc_run before luxb_init"); return LUXB_ERR_STATE; }
+  LUXB_ARG(is_tc_app(g->cfg.app), "luxb_tc_run needs a LUXB_TC handle (this one is app %d)", (int)g->cfg.app);
+  LUXB_CUDA(cudaSetDevice(g->cfg.device));
+  LUXB_CUDA(cudaEventRecord(g->ev_begin, g->stream));
+  LUXB_CUDA(cudaMemsetAsync(g->d_tc_t, 0, (size_t)g->nv * 8, g->stream));
+  LUXB_CUDA(cudaMemsetAsync(g->d_tc_next, 0, 8, g->stream));
+  const TcArgs a{g->d_tc_off, g->d_tc_dst, g->d_tc_staged, g->d_tc_stage_pre, g->d_tc_group, g->tc_n_group, g->d_tc_big, g->tc_n_big,
+                 g->d_tc_t, g->d_tc_next};
+  if (g->tc_n_group) {
+    tc_group_kernel<<<(int)std::min<uint32_t>(g->tc_n_group, g->tc_group_grid), kTcThreads, 0, g->stream>>>(a);
+    g->stats.kernel_launches++;
+  }
+  if (g->tc_n_big) {
+    tc_big_kernel<<<(int)std::min<uint32_t>(g->tc_n_big, g->tc_big_grid), kTcThreads, 0, g->stream>>>(a);
+    g->stats.kernel_launches++;
+  }
+  LUXB_CUDA(cudaGetLastError());
+  if (g->P > 1) LUXB_NCCL(nccl().AllReduce(g->d_tc_t, g->d_tc_t, g->nv, ncclUint64, ncclSum, g->comm, g->stream));
+  LUXB_CUDA(cub::DeviceReduce::Sum(g->d_tc_sum_tmp, g->tc_sum_bytes, g->d_tc_t, g->d_tc_total, (long long)g->nv, g->stream));
+  g->stats.iterations++;
+  g->stats.edges_processed += g->tc_m;
+  LUXB_TRY(finish_timed(g));
+  unsigned long long sum = 0;
+  LUXB_CUDA(cudaMemcpyAsync(&sum, g->d_tc_total, 8, cudaMemcpyDeviceToHost, g->stream));
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  if (total_out) *total_out = sum / 3;  // every triangle is in t at each of its three vertices
+  return 0;
+}
+
 // the array luxb_get_values / luxb_set_values address: label replica, current values, or betweenness scores
 static void* values_ptr(luxb_graph* g) {
   if (is_bc_app(g->cfg.app)) return g->d_scores;
+  if (is_tc_app(g->cfg.app)) return g->d_tc_t;
   return is_label_app(g->cfg.app) ? g->d_val[0] : g->d_val[g->cur];
 }
 
@@ -2808,6 +3015,7 @@ static int values_installed(luxb_graph* g, bool whole_array) {
 int luxb_set_values(luxb_graph* g, const void* host_in, size_t bytes) {
   LUXB_ARG(g && host_in, "NULL argument");
   if (!g->inited) { set_error("luxb_set_values before luxb_init"); return LUXB_ERR_STATE; }
+  LUXB_ARG(!is_tc_app(g->cfg.app), "luxb_set_values: triangle counts are computed from zero by luxb_tc_run");
   size_t need = (size_t)g->nv * g->vbytes;
   LUXB_ARG(bytes == need, "buffer is %zu bytes, vertex values need %zu", bytes, need);
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
@@ -2819,6 +3027,7 @@ int luxb_set_values(luxb_graph* g, const void* host_in, size_t bytes) {
 int luxb_set_local_values(luxb_graph* g, const void* host_in, size_t bytes) {
   LUXB_ARG(g && (host_in || g->n_part == 0), "NULL argument");
   if (!g->inited) { set_error("luxb_set_local_values before luxb_init"); return LUXB_ERR_STATE; }
+  LUXB_ARG(!is_tc_app(g->cfg.app), "luxb_set_local_values: triangle counts are computed from zero by luxb_tc_run");
   size_t need = (size_t)g->n_part * g->vbytes;
   LUXB_ARG(bytes == need, "buffer is %zu bytes, this rank's %u vertex values need %zu", bytes, g->n_part, need);
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
@@ -2831,6 +3040,7 @@ int luxb_check(luxb_graph* g, uint64_t* mistakes_out) {
   LUXB_ARG(g && mistakes_out, "NULL argument");
   if (!g->inited) { set_error("luxb_check before luxb_init"); return LUXB_ERR_STATE; }
   LUXB_ARG(!is_bc_app(g->cfg.app), "luxb_check: betweenness centrality has no check; it runs through luxb_bc_run");
+  LUXB_ARG(!is_tc_app(g->cfg.app), "luxb_check: triangle counting has no check; it runs through luxb_tc_run");
   LUXB_ARG(is_label_app(g->cfg.app),
            "the reference has no check for pagerank / col_filter (CHECK_TASK_ID is not registered in pull_model.inl:482-521)");
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
@@ -2970,7 +3180,8 @@ void luxb_close(luxb_graph* g) {
                   g->d_out_w, g->d_fq_all, g->d_fq_new, g->d_fq_tmp, g->d_hdr_all, g->d_counters, g->d_chunk_first, g->d_chunk_vtx,
                   g->d_partial, g->d_sync, g->d_hot_order, g->d_src_gather, g->d_hot, g->d_big_list, g->d_sigma, g->d_delta,
                   g->d_scores, g->d_order, g->d_bc_lvl, g->d_bc_off, g->d_bc_split, g->d_bc_sort_tmp, g->d_bc_ctl, g->d_bc_hubs,
-                  g->d_bc_partial};
+                  g->d_bc_partial, g->d_tc_off, g->d_tc_dst, g->d_tc_staged, g->d_tc_stage_pre, g->d_tc_group, g->d_tc_big,
+                  g->d_tc_t, g->d_tc_total, g->d_tc_next, g->d_tc_sum_tmp};
   for (void* p : ptrs) {
     if (!p) continue;
     if (std::find(g->host_allocs.begin(), g->host_allocs.end(), p) != g->host_allocs.end()) cudaFreeHost(p);

@@ -8,6 +8,7 @@
 #include "seg.cuh"
 #include "push.cuh"
 #include "bc.cuh"
+#include "tc.cuh"
 
 // fix-up scratch of one tiled sweep (pull.cuh): per-tile partials and carries, per-block aggregates
 struct FixupScratch {
@@ -177,6 +178,21 @@ struct luxb_graph {
   double* d_bc_partial = nullptr;
   std::vector<uint32_t> bc_off, bc_split;  // host copies of this source's level_off / split
   bool bc_has_source = false;
+  // triangle counting (tc.cuh): the oriented adjacency of the whole graph and the bins of this rank's range
+  uint64_t tc_m = 0;               // undirected simple edges
+  uint64_t* d_tc_off = nullptr;    // [nv + 1] out-list offsets
+  uint32_t* d_tc_dst = nullptr;    // [tc_m] out-lists N+(u), ascending ids
+  uint32_t* d_tc_staged = nullptr; // vertices of the grouped kernel
+  uint64_t* d_tc_stage_pre = nullptr;
+  uint32_t* d_tc_group = nullptr;
+  uint32_t* d_tc_big = nullptr;    // vertices of the big kernel
+  uint32_t tc_n_group = 0, tc_n_big = 0;
+  unsigned long long* d_tc_t = nullptr;  // [nv] per-vertex counts (the handle's values)
+  unsigned long long* d_tc_total = nullptr;  // [1] sum of t
+  unsigned int* d_tc_next = nullptr;         // [2] work counters
+  void* d_tc_sum_tmp = nullptr;
+  size_t tc_sum_bytes = 0;
+  int tc_group_grid = 0, tc_big_grid = 0;
 
   // communication
   luxb::ncclComm_t comm = nullptr;

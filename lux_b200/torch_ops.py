@@ -1,4 +1,4 @@
-"""PyTorch front-end of the C ABI (SURVEY §8 f4): the four Lux apps, weighted SSSP and betweenness centrality as `torch.ops.luxb.*` custom ops taking the CSC as
+"""PyTorch front-end of the C ABI (SURVEY §8 f4): the four Lux apps, weighted SSSP, betweenness centrality and triangle counting as `torch.ops.luxb.*` custom ops taking the CSC as
 torch tensors and returning torch tensors.  Plumbing only — every op opens a libluxb handle through the ctypes binding
 (lux_b200/binding.py), runs the app on the CUDA device of the current torch context and copies the result back; no torch
 kernel takes part in the computation, and there is no CPU fallback (the ops raise without a GPU).
@@ -11,6 +11,7 @@ kernel takes part in the computation, and there is no CPU fallback (the ops rais
     dist   = torch.ops.luxb.sssp_weighted(row_end, src, weight, 0)  # i64 [nv]  (weighted distance, INF = 2^32 - 1)
     bc     = torch.ops.luxb.betweenness(row_end, src, sources)  # f64 [nv]  (Σ over sources of Brandes' δ, not normalised)
     bc     = torch.ops.luxb.betweenness_weighted(row_end, src, weight, sources)  # f64 [nv]  (weighted paths, weights >= 1)
+    t      = torch.ops.luxb.triangles(row_end, src)             # i64 [nv]  (triangles at each vertex, undirected simple graph)
 row_end: int64 [nv] END offsets (the .lux convention); src: int64/int32 [ne]; weight: int32 [ne]; sources: int64/int32 [k] vertex ids."""
 import numpy as np
 import torch
@@ -34,6 +35,7 @@ _lib.define("colfilter(Tensor row_end, Tensor src, Tensor weight, int num_iter) 
 _lib.define("sssp_weighted(Tensor row_end, Tensor src, Tensor weight, int start) -> Tensor")
 _lib.define("betweenness(Tensor row_end, Tensor src, Tensor sources) -> Tensor")
 _lib.define("betweenness_weighted(Tensor row_end, Tensor src, Tensor weight, Tensor sources) -> Tensor")
+_lib.define("triangles(Tensor row_end, Tensor src) -> Tensor")
 
 
 def _pagerank(row_end, src, num_iter):
@@ -74,6 +76,12 @@ def _betweenness_weighted(row_end, src, weight, sources):
     return torch.from_numpy(out).to(row_end.device)
 
 
+def _triangles(row_end, src):
+    out = _apps.triangles(_np(row_end, np.uint64), _np(src, np.uint32), device=_device_index(row_end))
+    return torch.from_numpy(out["per_vertex"].astype(np.int64)).to(row_end.device)
+
+
 for _name, _fn in (("pagerank", _pagerank), ("components", _components), ("sssp", _sssp), ("colfilter", _colfilter),
-                   ("sssp_weighted", _sssp_weighted), ("betweenness", _betweenness), ("betweenness_weighted", _betweenness_weighted)):
+                   ("sssp_weighted", _sssp_weighted), ("betweenness", _betweenness), ("betweenness_weighted", _betweenness_weighted),
+                   ("triangles", _triangles)):
     _lib.impl(_name, _fn, "CompositeExplicitAutograd")
