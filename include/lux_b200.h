@@ -208,6 +208,10 @@ int luxb_partition_csc(luxb_vid nv, luxb_eid ne, const luxb_eid* row_end, int P,
 /* ---- communicator (replaces Legion's implicit zero-copy exchange, SURVEY §2.1) --------------------------- */
 int luxb_comm_unique_id(char id[LUXB_UNIQUE_ID_BYTES]);       /* rank 0; ship to the others out of band */
 int luxb_comm_init(luxb_graph* g, const char id[LUXB_UNIQUE_ID_BYTES]); /* collective; no-op when nranks == 1 */
+/* NCCL is bound at run time on the first of these two calls: the library named by the environment variable
+ * LUXB_NCCL_LIBRARY when it is set and loads, else libnccl.so.2, else libnccl.so.  It must export ncclGetUniqueId,
+ * ncclCommInitRank, ncclCommDestroy, ncclAllReduce, ncclBroadcast, ncclAllGather, ncclGroupStart, ncclGroupEnd and
+ * ncclGetErrorString; one binding serves the whole process. */
 /* P2P exchange: every rank exports its replica/frontier buffers (cudaIpcMemHandle), the caller all-gathers the
  * blobs (any transport) and hands the full table back. */
 int luxb_p2p_export(luxb_graph* g, void* blob, size_t* blob_bytes);

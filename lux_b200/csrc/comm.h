@@ -7,6 +7,7 @@
 #include <dlfcn.h>
 #include <stddef.h>
 #include <stdint.h>
+#include <stdlib.h>
 #include <mutex>
 
 namespace luxb {
@@ -31,13 +32,15 @@ struct NcclApi {
   const char* (*GetErrorString)(ncclResult_t) = nullptr;
 
   // returns nullptr on success, else a message.  Thread-safe: one host thread per GPU may race here.
+  // LUXB_NCCL_LIBRARY, when set, names the library to bind before libnccl.so.2 / libnccl.so are tried (another NCCL
+  // build, or a stand-in with the same nine entry points, such as the one-device rank emulation of the tests).
   const char* load() {
     static std::mutex mu;
     std::lock_guard<std::mutex> lock(mu);
     if (handle && GetErrorString) return nullptr;
-    const char* names[] = {"libnccl.so.2", "libnccl.so"};
+    const char* names[] = {getenv("LUXB_NCCL_LIBRARY"), "libnccl.so.2", "libnccl.so"};
     for (const char* n : names) {
-      handle = dlopen(n, RTLD_NOW | RTLD_GLOBAL);
+      if (n && *n) handle = dlopen(n, RTLD_NOW | RTLD_GLOBAL);
       if (handle) break;
     }
     if (!handle) return "cannot dlopen libnccl.so.2";
