@@ -10,6 +10,7 @@
   python apps/lux_cli.py bc         -weighted -file w.lux [-start v | -nsrc K -seed S] [-out scores.npy]
                                                                                    # weighted BC (i32 trailer, w >= 1; ours)
   python apps/lux_cli.py tc         -ng 1 -file g.lux [-out t.npy]                  # triangle counting (ours)
+  python apps/lux_cli.py kcore      -ng 1 -file g.lux [-check] [-out core.npy]      # k-core decomposition (ours)
   python apps/lux_cli.py converter  -nv N -ne M -input edges.txt -output g.lux     # tools/converter.cc:13-39 (host only)
 
 `-ll:gpu N` is accepted as a synonym of `-ng N` (README.md:47); -ll:fsize / -ll:zsize are accepted and ignored (HBM is
@@ -28,6 +29,11 @@ distance, every weight >= 1) with the same source flags.
 `tc` (no reference counterpart) counts the triangles of the graph read as undirected and simple (self-loops, parallel
 edges and both directions of an edge collapse; weights are ignored).  It prints "ELAPSED TIME" (device time of the count)
 and "TRIANGLES = T" on rank 0, and no "[Memory Setting]" line; `-out` saves the u64 triangle count of every vertex.
+
+`kcore` (no reference counterpart) computes the core number of every vertex of the same undirected simple graph.  It
+prints "ELAPSED TIME" (device time of the peel) and "DEGENERACY = K" (the largest core number) on rank 0, and no
+"[Memory Setting]" line; `-check` prints the check line above per rank (vertices that are not a fixpoint of the h-index
+operator); `-out` saves the u32 core numbers.
 """
 import os
 import subprocess
@@ -38,7 +44,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-APPS = {"pagerank": 0, "components": 1, "sssp": 2, "colfilter": 3, "bc": 5, "tc": 7}
+APPS = {"pagerank": 0, "components": 1, "sssp": 2, "colfilter": 3, "bc": 5, "tc": 7, "kcore": 8}
 
 
 def parse(argv):
@@ -160,7 +166,7 @@ def main():
     g = L.LuxGraph.from_file(opt["file"], app=weighted_app[app] if weighted else APPS[app], rank=rank, nranks=world, device=local,
                              start=opt["start"], verbose=opt["verbose"])
     b = g.bounds()
-    if rank == 0 and app not in ("bc", "tc"):
+    if rank == 0 and app not in ("bc", "tc", "kcore"):
         fb, zc = memory_setting(app, g.nv, g.ne, b, int(b["fq_right"][-1]) + 1, weighted)
         print("[Memory Setting] Set ll:fsize >= %dMB and ll:zsize >= %dMB" % (fb, zc), flush=True)
     g.comm_init_torch()
@@ -171,13 +177,17 @@ def main():
         g.bc_run(bc_sources(opt, g.nv))
     elif app == "tc":
         total = g.tc_run()
+    elif app == "kcore":
+        degeneracy = g.kcore_run()
     else:
         g.run_to_convergence()
     if rank == 0:
         print("ELAPSED TIME = %7.7f s" % g.stats()["loop_seconds"], flush=True)
         if app == "tc":
             print("TRIANGLES = %d" % total, flush=True)
-    if opt["check"] and app in ("components", "sssp"):
+        if app == "kcore":
+            print("DEGENERACY = %d" % degeneracy, flush=True)
+    if opt["check"] and app in ("components", "sssp", "kcore"):
         bad = g.check()
         print("[%s] Check task: rowLeft(%u) numMistakes(%u)" % ("PASS" if bad == 0 else "FAIL", int(b["row_left"][rank]), bad),
               flush=True)

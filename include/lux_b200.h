@@ -54,8 +54,10 @@ typedef enum {
                             f64 score per vertex; runs through luxb_bc_run */
   LUXB_BC_WEIGHTED = 6,  /* weighted betweenness centrality (no reference counterpart) — Brandes over the weighted SSSP
                             distances (weights >= 1), f64 score per vertex; runs through luxb_bc_run */
-  LUXB_TC = 7            /* triangle counting (no reference counterpart) — exact u64 count of the triangles at every
+  LUXB_TC = 7,           /* triangle counting (no reference counterpart) — exact u64 count of the triangles at every
                             vertex of the undirected simple graph; runs through luxb_tc_run */
+  LUXB_KCORE = 8         /* k-core decomposition (no reference counterpart) — exact u32 core number of every vertex of
+                            the undirected simple graph, by level-synchronous peeling; runs through luxb_kcore_run */
 } luxb_app;
 
 /* Weighted SSSP (LUXB_SSSP_WEIGHTED):
@@ -120,6 +122,31 @@ typedef enum {
  * luxb_check return LUXB_ERR_ARG.  luxb_stats: iterations = luxb_tc_run calls, edges_processed += m (undirected simple
  * edges) per call, loop_seconds = device time of the luxb_tc_run calls.  luxb_get_local_csc / luxb_device_view keep
  * returning this rank's CSC slice.  cfg.start_vtx, cfg.exchange and cfg.verbose have no effect. */
+
+/* k-core decomposition (LUXB_KCORE).  The graph is LUXB_TC's: {u, v} is an edge iff u != v and u -> v or v -> u is
+ * stored (parallel edges, both directions and self-loops collapse; weights are ignored, a weighted CSC is accepted);
+ * deg(v) is the number of distinct neighbours.
+ *  - core[v] (u32) is the largest k such that v lies in a subgraph whose every vertex has degree >= k (networkx's
+ *    core_number() on the simple graph).  Isolated vertices, self-loops only included, have core 0.  The degeneracy is
+ *    the largest core number (0 on a graph without edges).
+ *  - The peel: k = 0; while a vertex is alive: k = max(k, min deg over the alive vertices); repeat: F = {alive v :
+ *    deg(v) <= k}, stop if F is empty, core[F] = k, remove F and lower the degrees of the remaining vertices.  A round
+ *    is one non-empty F, a level one value of k with at least one round.  The rounds' sets do not depend on the
+ *    schedule or on the number of ranks; integers only, so neither does anything else.
+ * luxb_init builds, on every rank, the lists of this rank's neighbours of every vertex (each adjacency entry of the
+ * graph is held by exactly one rank).  The handle's values (luxb_get_values / luxb_get_local_values) are the core
+ * numbers, 4 bytes per vertex: zeros before the first luxb_kcore_run, complete on every rank after one.
+ * luxb_set_values / luxb_set_local_values overwrite them so that luxb_check can judge any assignment; the next
+ * luxb_kcore_run recomputes them.  luxb_iterate and luxb_run_to_convergence return LUXB_ERR_ARG.
+ * luxb_check counts this rank's vertices v that are not a fixpoint of the h-index operator: with c = core[v],
+ * a = |{u in N(v) : core[u] >= c}| and b = |{u in N(v) : core[u] >= c + 1}|, v is a violation iff a < c or b >= c + 1.
+ * True core numbers always pass: v lies in its own c-core, so a >= c; and if b >= c + 1, v and its neighbours of core
+ * >= c + 1 would form a subgraph of min degree >= c + 1, putting v in the (c + 1)-core.  Passing is necessary, not
+ * sufficient: the core numbers are the LARGEST fixpoint, and all zeros pass as well.
+ * luxb_stats: iterations += rounds, edges_processed += 2m (the adjacency entries scanned, summed over the ranks: the
+ * same figure on every rank), loop_seconds = device time of the run.  luxb_trace holds the last run, one entry per
+ * round: active = |F| over all ranks, pull = that round's k.  cfg.start_vtx, cfg.exchange, cfg.verbose and
+ * cfg.balanced_split have no effect: the work split is the reference's (luxb_work_bounds says so). */
 
 typedef enum {
   LUXB_EXCHANGE_NCCL = 0, /* library collectives only: PageRank packs its share and broadcasts the two ranges of every
@@ -239,7 +266,7 @@ int luxb_iterate(luxb_graph* g, int iters, uint64_t* active_out);
 int luxb_run_to_convergence(luxb_graph* g, int max_iters, int* iters_out);
 
 /* ---- results / check / stats -------------------------------------------------------------------------------- */
-/* Full vertex-value array (what the reference holds in dist_lr[iter%2]): nv * {4 | 4 | 80 | 8 (BC scores, TC counts)} bytes.  PageRank on
+/* Full vertex-value array (what the reference holds in dist_lr[iter%2]): nv * {4 | 4 | 80 | 8 (BC scores, TC counts) | 4 (core numbers)} bytes.  PageRank on
  * nranks > 1 exchanges only the values that are ever gathered each iteration and completes the full array on demand:
  * there the call is collective (every rank calls it at the same point). */
 int luxb_get_values(luxb_graph* g, void* host_out, size_t bytes);
@@ -317,6 +344,12 @@ int luxb_bc_source_state(luxb_graph* g, uint32_t* lev, double* sigma, double* de
  * nranks > 1: each rank counts the triangles found at the vertices of its own range, then t is summed over the ranks.
  * LUXB_ERR_STATE before luxb_init, LUXB_ERR_ARG on another app. */
 int luxb_tc_run(luxb_graph* g, uint64_t* total_out);
+
+/* ---- k-core decomposition (LUXB_KCORE handles) -------------------------------------------------------------------- */
+/* Recompute every core number from scratch (the handle's values) and write the degeneracy to *degeneracy_out (may be
+ * NULL).  Collective on nranks > 1: each rank peels its own range, the pieces of every round's F are exchanged, and the
+ * core numbers are completed on every rank at the end.  LUXB_ERR_STATE before luxb_init, LUXB_ERR_ARG on another app. */
+int luxb_kcore_run(luxb_graph* g, uint32_t* degeneracy_out);
 
 void luxb_close(luxb_graph* g);
 const char* luxb_last_error(void);

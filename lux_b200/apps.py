@@ -7,11 +7,12 @@ colfilter  : col_filter/colfilter.cc:71-81    (-ni fixed iterations)
 betweenness: Brandes from a list of sources over the SSSP engine's hop levels, or with weights over the weighted
              SSSP distances (ours; the reference has no BC)
 triangles  : exact triangle counts of the undirected simple graph (ours)
+core_number: exact core numbers of the undirected simple graph, by level-synchronous peeling (ours)
 Single-rank convenience wrappers; multi-GPU callers drive LuxGraph directly (see bench.py).
 """
 import numpy as np
 
-from .binding import LuxGraph, APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC, APP_BC_WEIGHTED, APP_TC
+from .binding import LuxGraph, APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC, APP_BC_WEIGHTED, APP_TC, APP_KCORE
 
 
 def pagerank(row_end, src, num_iter=10, device=0):
@@ -74,3 +75,13 @@ def triangles(row_end, src, device=0):
         g.init()
         total = g.tc_run()
         return dict(total=total, per_vertex=g.values())
+
+
+def core_number(row_end, src, device=0):
+    """Core numbers of the CSC read as an undirected simple graph ({u, v} is an edge iff u != v and u -> v or v -> u is
+    stored; weights are ignored), as networkx's core_number(): dict(core = u32 [nv], degeneracy = the largest core
+    number, rounds = the peel's rounds)."""
+    with LuxGraph.from_csc(row_end, src, app=APP_KCORE, device=device) as g:
+        g.init()
+        degeneracy = g.kcore_run()
+        return dict(core=g.values(), degeneracy=degeneracy, rounds=g.stats()["iterations"])

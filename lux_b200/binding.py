@@ -6,7 +6,7 @@ import numpy as np
 
 from . import build as _build
 
-APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC, APP_BC_WEIGHTED, APP_TC = 0, 1, 2, 3, 4, 5, 6, 7
+APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC, APP_BC_WEIGHTED, APP_TC, APP_KCORE = 0, 1, 2, 3, 4, 5, 6, 7, 8
 DIST_INF = 0xFFFFFFFF  # APP_SSSP_WEIGHTED / APP_BC_WEIGHTED: distance of an unreachable vertex (LUXB_DIST_INF)
 EXCHANGE_NCCL, EXCHANGE_P2P, EXCHANGE_P2P_FUSED = 0, 1, 2
 DENSE_BITMAP, SPARSE_QUEUE = 0x1234567, 0x7654321
@@ -121,7 +121,7 @@ def convert_edgelist(edge_list_path, lux_path, nv, ne):
 
 _VDTYPE = {APP_PAGERANK: np.float32, APP_CC: np.uint32, APP_SSSP: np.uint32, APP_COLFILTER: np.float32,
            APP_SSSP_WEIGHTED: np.uint32, APP_BC: np.float64, APP_BC_WEIGHTED: np.float64,
-           APP_TC: np.uint64}
+           APP_TC: np.uint64, APP_KCORE: np.uint32}
 
 
 class LuxGraph:
@@ -335,6 +335,14 @@ class LuxGraph:
         total = C.c_uint64(0)
         _chk(load_library().luxb_tc_run(self._h, C.byref(total)), "luxb_tc_run")
         return total.value
+
+    def kcore_run(self):
+        """k-core decomposition (APP_KCORE handles): recompute the core number of every vertex of the undirected simple
+        graph (the u32 values() returns) and return the degeneracy (the largest core number).  Collective on
+        nranks > 1."""
+        degeneracy = C.c_uint32(0)
+        _chk(load_library().luxb_kcore_run(self._h, C.byref(degeneracy)), "luxb_kcore_run")
+        return degeneracy.value
 
     def enable_kernel_timing(self, on=True):
         _chk(load_library().luxb_enable_kernel_timing(self._h, C.c_int(1 if on else 0)), "luxb_enable_kernel_timing")

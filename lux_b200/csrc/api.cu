@@ -23,6 +23,8 @@ using namespace luxb;
 static bool is_bc_app(luxb_app app) { return app == LUXB_BC || app == LUXB_BC_WEIGHTED; }
 // triangle counting: luxb_tc_run instead of luxb_iterate, u64 counts as values
 static bool is_tc_app(luxb_app app) { return app == LUXB_TC; }
+// k-core decomposition: luxb_kcore_run instead of luxb_iterate, u32 core numbers as values
+static bool is_kcore_app(luxb_app app) { return app == LUXB_KCORE; }
 // labels are weighted distances (u32, INF = LUXB_DIST_INF, label_iteration<WeightedDistProgram>): the app reads the CSC
 // weights, keeps out_w beside the push CSR and pulls through the merge-path sweep only
 static bool weighted_labels(luxb_app app) { return app == LUXB_SSSP_WEIGHTED || app == LUXB_BC_WEIGHTED; }
@@ -247,7 +249,7 @@ static bool use_balanced_split(const luxb_config* cfg) {
 
 static int check_config(const luxb_config* cfg) {
   LUXB_ARG(cfg != nullptr, "config is NULL");
-  LUXB_ARG(cfg->app >= LUXB_PAGERANK && cfg->app <= LUXB_TC, "unknown app %d", (int)cfg->app);
+  LUXB_ARG(cfg->app >= LUXB_PAGERANK && cfg->app <= LUXB_KCORE, "unknown app %d", (int)cfg->app);
   LUXB_ARG(cfg->nranks >= 1 && cfg->nranks <= LUXB_MAX_PARTS, "nranks %d out of range [1,%d]", cfg->nranks, LUXB_MAX_PARTS);
   LUXB_ARG(cfg->rank >= 0 && cfg->rank < cfg->nranks, "rank %d out of range", cfg->rank);
   return 0;
@@ -1124,6 +1126,7 @@ static int pagerank_publish(luxb_graph* g, float* x_new);
 static int wait_cold_exchange(luxb_graph* g);
 static int bc_alloc(luxb_graph* g);
 static int tc_build(luxb_graph* g);
+static int kcore_build(luxb_graph* g);
 
 // The gather side of the pull sweeps: global out-degrees, the hot set (build_hot_layout), the flagged streams if
 // `streams` (build_seg_sweep) and the hot copies Z = [hot | compact cold values on one rank] + one whole table of slack:
@@ -1233,6 +1236,11 @@ int luxb_init(luxb_graph* g) {
     case LUXB_TC: {
       g->vbytes = 8;
       LUXB_TRY(tc_build(g));
+      break;
+    }
+    case LUXB_KCORE: {
+      g->vbytes = 4;
+      LUXB_TRY(kcore_build(g));
       break;
     }
   }
@@ -2454,6 +2462,7 @@ int luxb_iterate(luxb_graph* g, int iters, uint64_t* active_out) {
   if (!g->inited) { set_error("luxb_iterate before luxb_init"); return LUXB_ERR_STATE; }
   LUXB_ARG(!is_bc_app(g->cfg.app), "luxb_iterate: betweenness centrality runs through luxb_bc_run");
   LUXB_ARG(!is_tc_app(g->cfg.app), "luxb_iterate: triangle counting runs through luxb_tc_run");
+  LUXB_ARG(!is_kcore_app(g->cfg.app), "luxb_iterate: k-core decomposition runs through luxb_kcore_run");
   LUXB_ARG(iters >= 0, "negative iteration count");
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
   if (const char* env = getenv("LUXB_PHASE_TIMING")) { g->pt.on = atoi(env) != 0; g->pt.per_call = atoi(env) == 2; }  // may change between calls
@@ -2472,6 +2481,7 @@ int luxb_run_to_convergence(luxb_graph* g, int max_iters, int* iters_out) {
   if (!g->inited) { set_error("luxb_run_to_convergence before luxb_init"); return LUXB_ERR_STATE; }
   LUXB_ARG(!is_bc_app(g->cfg.app), "luxb_run_to_convergence: betweenness centrality runs through luxb_bc_run");
   LUXB_ARG(!is_tc_app(g->cfg.app), "luxb_run_to_convergence: triangle counting runs through luxb_tc_run");
+  LUXB_ARG(!is_kcore_app(g->cfg.app), "luxb_run_to_convergence: k-core decomposition runs through luxb_kcore_run");
   LUXB_ARG(is_label_app(g->cfg.app), "only push apps converge (pagerank/col_filter run -ni iterations)");
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
   LUXB_CUDA(cudaEventRecord(g->ev_begin, g->stream));
@@ -2782,15 +2792,11 @@ static int tc_sort_unique(luxb_graph* g, DevTmp& tmp, uint64_t* keys, uint64_t* 
   return 0;
 }
 
-// luxb_init of a LUXB_TC handle: the undirected simple edges of the whole graph (on several ranks every rank's distinct
-// keys go to every rank), the oriented out-lists, the work per vertex and the bins of this rank's range
-static int tc_build(luxb_graph* g) {
-  DevTmp tmp;
+// The distinct undirected keys min << 32 | max of the whole graph, on every rank (on several ranks every rank's distinct
+// keys go to every rank), at the front of *keys; *alt is a buffer of the same size.  Both belong to `tmp`.  The graph of
+// LUXB_TC and LUXB_KCORE.
+static int undirected_keys(luxb_graph* g, DevTmp& tmp, int bits, uint64_t** keys_out, uint64_t** alt_out, uint64_t* m_out) {
   const int grid = g->num_sms * 8;
-  const uint32_t nv = g->nv;
-  int vbits = 1;
-  while ((1ull << vbits) < (uint64_t)nv) ++vbits;
-  const int bits = 32 + vbits;  // min < nv in the high word, max in the low one
   uint64_t *d_keys = nullptr, *d_alt = nullptr;
   unsigned long long* d_cur = nullptr;
   LUXB_TRY(tmp.alloc(&d_keys, g->e_part));
@@ -2833,6 +2839,29 @@ static int tc_build(luxb_graph* g) {
     d_alt = d_all_alt;
     LUXB_TRY(tc_sort_unique(g, tmp, d_keys, d_alt, total, bits, &m));
   }
+  *keys_out = d_keys;
+  *alt_out = d_alt;
+  *m_out = m;
+  return 0;
+}
+
+// bits of a sort key (high word) << 32 | (low word) over vertex ids < nv
+static int pair_key_bits(uint32_t nv) {
+  int vbits = 1;
+  while ((1ull << vbits) < (uint64_t)nv) ++vbits;
+  return 32 + vbits;
+}
+
+// luxb_init of a LUXB_TC handle: the undirected simple edges of the whole graph (undirected_keys), the oriented
+// out-lists, the work per vertex and the bins of this rank's range
+static int tc_build(luxb_graph* g) {
+  DevTmp tmp;
+  const int grid = g->num_sms * 8;
+  const uint32_t nv = g->nv;
+  const int bits = pair_key_bits(nv);  // min < nv in the high word, max in the low one
+  uint64_t *d_keys = nullptr, *d_alt = nullptr;
+  uint64_t m = 0;
+  LUXB_TRY(undirected_keys(g, tmp, bits, &d_keys, &d_alt, &m));
   g->tc_m = m;
   // degrees, orientation, out-lists sorted by (from, to), offsets and the work W(u)
   uint32_t *d_deg = nullptr, *d_outdeg = nullptr;
@@ -2954,10 +2983,203 @@ int luxb_tc_run(luxb_graph* g, uint64_t* total_out) {
   return 0;
 }
 
-// the array luxb_get_values / luxb_set_values address: label replica, current values, or betweenness scores
+// ---- k-core decomposition (kcore.cuh) ------------------------------------------------------------------------------
+// luxb_init of a LUXB_KCORE handle: the undirected keys (undirected_keys, as for TC), then this rank's adjacency: the
+// entries a -> b of every key {a, b} whose b is this rank's, sorted by (a, b) into a CSR over all nv sources
+static int kcore_build(luxb_graph* g) {
+  DevTmp tmp;
+  const int grid = g->num_sms * 8;
+  const uint32_t nv = g->nv, n_part = g->n_part;
+  const int bits = pair_key_bits(nv);
+  uint64_t *d_keys = nullptr, *d_alt = nullptr, m = 0;
+  LUXB_TRY(undirected_keys(g, tmp, bits, &d_keys, &d_alt, &m));
+  g->kc_m = m;
+  tmp.release(d_alt);
+  // this rank's entries: counted first, so that the two sort buffers hold this rank's share (2m / P on average), and
+  // the keys go before the second buffer is allocated
+  uint64_t *d_ent = nullptr, *d_ent_alt = nullptr;
+  unsigned long long* d_cur = nullptr;
+  LUXB_TRY(tmp.alloc(&d_cur, 1));
+  const uint32_t row_right = n_part ? g->row_left + n_part - 1 : 0;
+  unsigned long long n_ent = 0;
+  for (int pass = 0; pass < 2; ++pass) {
+    if (pass == 1) LUXB_TRY(tmp.alloc(&d_ent, n_ent));
+    LUXB_CUDA(cudaMemsetAsync(d_cur, 0, 8, g->stream));
+    if (m && n_part) kcore_emit_kernel<<<grid_for(m, 256, grid), 256, 0, g->stream>>>(d_keys, m, g->row_left, row_right, d_cur, d_ent);
+    LUXB_CUDA(cudaGetLastError());
+    LUXB_CUDA(cudaMemcpyAsync(&n_ent, d_cur, 8, cudaMemcpyDeviceToHost, g->stream));
+    LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  }
+  tmp.release(d_keys);
+  LUXB_TRY(tmp.alloc(&d_ent_alt, n_ent));
+  const uint64_t* d_sorted = d_ent;
+  if (n_ent) {
+    cub::DoubleBuffer<uint64_t> db(d_ent, d_ent_alt);
+    LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+      return cub::DeviceRadixSort::SortKeys(t, b, db, (long long)n_ent, 0, bits, g->stream);
+    }));
+    d_sorted = db.Current();
+  }
+  uint32_t* d_len = nullptr;
+  LUXB_TRY(tmp.alloc(&d_len, nv));
+  LUXB_CUDA(cudaMemsetAsync(d_len, 0, (size_t)nv * 4, g->stream));
+  LUXB_TRY(dmalloc(&g->d_kc_deg0, n_part));
+  LUXB_CUDA(cudaMemsetAsync(g->d_kc_deg0, 0, (size_t)n_part * 4, g->stream));
+  LUXB_TRY(dmalloc(&g->d_kc_adj, n_ent));
+  if (n_ent)
+    kcore_lists_kernel<<<grid_for(n_ent, 256, grid), 256, 0, g->stream>>>(d_sorted, n_ent, g->row_left, g->d_kc_adj, d_len, g->d_kc_deg0);
+  LUXB_CUDA(cudaGetLastError());
+  LUXB_TRY(dmalloc(&g->d_kc_off, (uint64_t)nv + 1));
+  LUXB_CUDA(cudaMemsetAsync(g->d_kc_off + nv, 0, 8, g->stream));
+  widen_u32_to_u64_kernel<<<grid_for(nv, 256, grid), 256, 0, g->stream>>>(d_len, g->d_kc_off, nv);
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceScan::ExclusiveSum(t, b, g->d_kc_off, g->d_kc_off, (long long)nv + 1, g->stream);
+  }));
+  // the run's state: core (zeros until the first run), degrees, alive lists, pieces, F, its slot offsets, records
+  LUXB_TRY(dmalloc(&g->d_kc_core, nv));
+  LUXB_CUDA(cudaMemsetAsync(g->d_kc_core, 0, (size_t)nv * 4, g->stream));
+  LUXB_TRY(dmalloc(&g->d_kc_deg, 2 * (uint64_t)n_part));
+  for (int i = 0; i < 2; ++i) {
+    LUXB_TRY(dmalloc(&g->d_kc_alive[i], n_part));
+    LUXB_TRY(dmalloc(&g->d_kc_piece[i], n_part));
+  }
+  if (g->P > 1) LUXB_TRY(dmalloc(&g->d_kc_f, nv));
+  LUXB_TRY(dmalloc(&g->d_kc_pre, (uint64_t)nv + 1));
+  LUXB_TRY(dmalloc(&g->d_kc_rec, 1 + LUXB_MAX_PARTS));
+  LUXB_CUDA(cudaMallocHost(&g->h_kc_rec, LUXB_MAX_PARTS * sizeof(KcoreRec)));
+  LUXB_TRY(dmalloc(&g->d_kc_bad, 1));
+  LUXB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, g->kc_scan_bytes, g->d_kc_pre, g->d_kc_pre, (long long)nv + 1, g->stream));
+  LUXB_TRY(dmalloc((char**)&g->d_kc_scan_tmp, g->kc_scan_bytes));
+  int per_sm = 0, per_sm2 = 0;
+  LUXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kcore_scatter_kernel, kKcoreThreads, 0));
+  LUXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm2, kcore_tally_kernel, kKcoreThreads, 0));
+  g->kc_grid = std::max(std::min(per_sm, per_sm2), 1) * g->num_sms;
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  return 0;
+}
+
+int luxb_kcore_run(luxb_graph* g, uint32_t* degeneracy_out) {
+  LUXB_ARG(g != nullptr, "graph is NULL");
+  if (!g->inited) { set_error("luxb_kcore_run before luxb_init"); return LUXB_ERR_STATE; }
+  LUXB_ARG(is_kcore_app(g->cfg.app), "luxb_kcore_run needs a LUXB_KCORE handle (this one is app %d)", (int)g->cfg.app);
+  LUXB_CUDA(cudaSetDevice(g->cfg.device));
+  LUXB_CUDA(cudaEventRecord(g->ev_begin, g->stream));
+  const uint32_t n_part = g->n_part, P = (uint32_t)g->P;
+  const int grid = grid_for(std::max<uint32_t>(n_part, 1), 256, g->num_sms * 8);
+  KcoreRec* rec = g->d_kc_rec;
+  // every own vertex alive; core stays zero outside this rank's range, so that a sum completes it at the end
+  LUXB_CUDA(cudaMemsetAsync(g->d_kc_core, 0, (size_t)g->nv * 4, g->stream));
+  kcore_reset_kernel<<<grid, 256, 0, g->stream>>>(g->d_kc_core, g->d_kc_deg, g->d_kc_deg0, g->d_kc_alive[0], n_part, g->row_left, rec);
+  kcore_tally_kernel<<<std::min(grid, g->kc_grid), kKcoreThreads, 0, g->stream>>>(g->d_kc_alive[0], n_part, g->d_kc_core, g->d_kc_deg,
+                                                                                   g->row_left, g->d_kc_alive[1], rec);
+  g->stats.kernel_launches += 2;
+  LUXB_CUDA(cudaGetLastError());
+  g->trace_active.clear();
+  g->trace_pull.clear();
+  int alive_cur = 0, piece_cur = 0;  // the first tally reads alive[0]
+  uint32_t n_alive = 0, k = 0;
+  uint64_t rounds = 0;
+  std::vector<uint32_t> piece(P);
+  for (;;) {
+    // the one host synchronisation of a round: every rank's record
+    if (P > 1) LUXB_NCCL(nccl().AllGather(rec, rec + 1, sizeof(KcoreRec), ncclUint8, g->comm, g->stream));
+    LUXB_CUDA(cudaMemcpyAsync(g->h_kc_rec, P > 1 ? rec + 1 : rec, P * sizeof(KcoreRec), cudaMemcpyDeviceToHost, g->stream));
+    LUXB_CUDA(cudaStreamSynchronize(g->stream));
+    const KcoreRec* r = g->h_kc_rec;
+    if (!r[g->cfg.rank].next) {  // the tally ran on this rank (kcore_tally_kernel): its compacted list is current
+      alive_cur ^= 1;
+      n_alive = r[g->cfg.rank].alive;
+    }
+    uint64_t next = 0, alive = 0;
+    for (uint32_t p = 0; p < P; ++p) { next += r[p].next; alive += r[p].alive; }
+    const uint32_t* own = g->d_kc_piece[piece_cur ^ 1];
+    if (next) {  // the level goes on: the pieces the scatter appended
+      for (uint32_t p = 0; p < P; ++p) piece[p] = r[p].next;
+    } else {     // a new level: k = the least degree left, its first pieces the alive vertices at that degree
+      if (!alive) break;
+      uint32_t least = kKcoreUnset;
+      for (uint32_t p = 0; p < P; ++p)
+        if (r[p].alive) least = std::min(least, (uint32_t)(r[p].min_cnt >> 32));
+      k = std::max(k, least);
+      for (uint32_t p = 0; p < P; ++p) piece[p] = r[p].alive && (uint32_t)(r[p].min_cnt >> 32) == k ? (uint32_t)r[p].min_cnt : 0;
+      if (piece[g->cfg.rank]) {
+        kcore_select_kernel<<<grid_for(n_alive, 256, g->num_sms * 8), 256, 0, g->stream>>>(
+            g->d_kc_alive[alive_cur], n_alive, g->d_kc_deg, g->row_left, k, g->d_kc_piece[piece_cur ^ 1], rec);
+        g->stats.kernel_launches++;
+      }
+    }
+    piece_cur ^= 1;
+    uint64_t nf = 0;
+    for (uint32_t p = 0; p < P; ++p) nf += piece[p];
+    if (!nf) {  // every rank sees the same records, so every rank stops here: a round that removes nothing never ends
+      set_error("luxb_kcore_run: round %llu at k = %u has an empty frontier with %llu vertices alive",
+                (unsigned long long)rounds, k, (unsigned long long)alive);
+      return LUXB_ERR_STATE;
+    }
+    const uint32_t mine = piece[g->cfg.rank];
+    kcore_mark_kernel<<<grid_for(std::max<uint32_t>(mine, 1), 256, g->num_sms * 8), 256, 0, g->stream>>>(own, mine, k, g->d_kc_core, rec);
+    g->stats.kernel_launches++;
+    const uint32_t* f = own;
+    if (P > 1) {  // the pieces in rank order, the same empty ones skipped on every rank
+      LUXB_NCCL(nccl().GroupStart());
+      uint64_t at = 0;
+      for (uint32_t p = 0; p < P; ++p) {
+        if (piece[p])
+          LUXB_NCCL(nccl().Broadcast(p == (uint32_t)g->cfg.rank ? own : g->d_kc_f + at, g->d_kc_f + at, piece[p], ncclUint32, (int)p, g->comm, g->stream));
+        at += piece[p];
+      }
+      LUXB_NCCL(nccl().GroupEnd());
+      f = g->d_kc_f;
+    }
+    kcore_lengths_kernel<<<grid_for(nf + 1, 256, g->num_sms * 8), 256, 0, g->stream>>>(f, (uint32_t)nf, g->d_kc_off, g->d_kc_pre);
+    size_t scan_bytes = 0;
+    LUXB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, g->d_kc_pre, g->d_kc_pre, (long long)nf + 1, g->stream));
+    LUXB_ARG(scan_bytes <= g->kc_scan_bytes, "k-core scan needs %zu bytes of temporary storage, %zu reserved", scan_bytes, g->kc_scan_bytes);
+    LUXB_CUDA(cub::DeviceScan::ExclusiveSum(g->d_kc_scan_tmp, scan_bytes, g->d_kc_pre, g->d_kc_pre, (long long)nf + 1, g->stream));
+    const KcoreScatterArgs sa{f, (uint32_t)nf, g->d_kc_pre, g->d_kc_off, g->d_kc_adj, g->d_kc_core, g->d_kc_deg, g->row_left, k,
+                              g->d_kc_piece[piece_cur ^ 1], rec};
+    kcore_scatter_kernel<<<g->kc_grid, kKcoreThreads, 0, g->stream>>>(sa);
+    kcore_tally_kernel<<<std::min(grid_for(std::max<uint32_t>(n_alive, 1), kKcoreThreads, g->num_sms * 8), g->kc_grid), kKcoreThreads, 0,
+                         g->stream>>>(g->d_kc_alive[alive_cur], n_alive, g->d_kc_core, g->d_kc_deg, g->row_left,
+                                      g->d_kc_alive[alive_cur ^ 1], rec);
+    g->stats.kernel_launches += 4;  // the scan counts as one
+    LUXB_CUDA(cudaGetLastError());
+    g->trace_active.push_back(nf);
+    g->trace_pull.push_back((int32_t)k);
+    ++rounds;
+  }
+  // every rank holds its own range; zeros elsewhere, so a sum completes core everywhere
+  if (P > 1) LUXB_NCCL(nccl().AllReduce(g->d_kc_core, g->d_kc_core, g->nv, ncclUint32, ncclSum, g->comm, g->stream));
+  g->stats.iterations += rounds;
+  g->stats.edges_processed += 2 * g->kc_m;
+  LUXB_TRY(finish_timed(g));
+  if (degeneracy_out) *degeneracy_out = k;
+  return 0;
+}
+
+// luxb_check of a LUXB_KCORE handle: this rank's vertices that are not a fixpoint of the h-index operator
+static int kcore_check(luxb_graph* g, uint64_t* mistakes_out) {
+  const int grid = g->num_sms * 8;
+  LUXB_CUDA(cudaMemsetAsync(g->d_kc_bad, 0, 8, g->stream));
+  LUXB_CUDA(cudaMemsetAsync(g->d_kc_deg, 0, (size_t)g->n_part * 8, g->stream));
+  if (g->n_part) {
+    kcore_check_count_kernel<<<grid, 256, 0, g->stream>>>(g->d_kc_off, g->d_kc_adj, g->nv, g->d_kc_core, g->row_left, g->n_part, g->d_kc_deg);
+    kcore_check_kernel<<<grid_for(g->n_part, 256, grid), 256, 0, g->stream>>>(g->d_kc_core, g->row_left, g->n_part, g->d_kc_deg, g->d_kc_bad);
+    LUXB_CUDA(cudaGetLastError());
+  }
+  unsigned long long bad = 0;
+  LUXB_CUDA(cudaMemcpyAsync(&bad, g->d_kc_bad, 8, cudaMemcpyDeviceToHost, g->stream));
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  *mistakes_out = bad;
+  return 0;
+}
+
+// the array luxb_get_values / luxb_set_values address: label replica, current values, betweenness scores, triangle
+// counts or core numbers
 static void* values_ptr(luxb_graph* g) {
   if (is_bc_app(g->cfg.app)) return g->d_scores;
   if (is_tc_app(g->cfg.app)) return g->d_tc_t;
+  if (is_kcore_app(g->cfg.app)) return g->d_kc_core;
   return is_label_app(g->cfg.app) ? g->d_val[0] : g->d_val[g->cur];
 }
 
@@ -3041,6 +3263,10 @@ int luxb_check(luxb_graph* g, uint64_t* mistakes_out) {
   if (!g->inited) { set_error("luxb_check before luxb_init"); return LUXB_ERR_STATE; }
   LUXB_ARG(!is_bc_app(g->cfg.app), "luxb_check: betweenness centrality has no check; it runs through luxb_bc_run");
   LUXB_ARG(!is_tc_app(g->cfg.app), "luxb_check: triangle counting has no check; it runs through luxb_tc_run");
+  if (is_kcore_app(g->cfg.app)) {
+    LUXB_CUDA(cudaSetDevice(g->cfg.device));
+    return kcore_check(g, mistakes_out);
+  }
   LUXB_ARG(is_label_app(g->cfg.app),
            "the reference has no check for pagerank / col_filter (CHECK_TASK_ID is not registered in pull_model.inl:482-521)");
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
@@ -3181,7 +3407,9 @@ void luxb_close(luxb_graph* g) {
                   g->d_partial, g->d_sync, g->d_hot_order, g->d_src_gather, g->d_hot, g->d_big_list, g->d_sigma, g->d_delta,
                   g->d_scores, g->d_order, g->d_bc_lvl, g->d_bc_off, g->d_bc_split, g->d_bc_sort_tmp, g->d_bc_ctl, g->d_bc_hubs,
                   g->d_bc_partial, g->d_tc_off, g->d_tc_dst, g->d_tc_staged, g->d_tc_stage_pre, g->d_tc_group, g->d_tc_big,
-                  g->d_tc_t, g->d_tc_total, g->d_tc_next, g->d_tc_sum_tmp};
+                  g->d_tc_t, g->d_tc_total, g->d_tc_next, g->d_tc_sum_tmp, g->d_kc_off, g->d_kc_adj, g->d_kc_deg0, g->d_kc_deg,
+                  g->d_kc_core, g->d_kc_alive[0], g->d_kc_alive[1], g->d_kc_piece[0], g->d_kc_piece[1], g->d_kc_f, g->d_kc_pre,
+                  g->d_kc_rec, g->d_kc_bad, g->d_kc_scan_tmp};
   for (void* p : ptrs) {
     if (!p) continue;
     if (std::find(g->host_allocs.begin(), g->host_allocs.end(), p) != g->host_allocs.end()) cudaFreeHost(p);
@@ -3199,6 +3427,7 @@ void luxb_close(luxb_graph* g) {
   if (g->h_barrier_err) cudaFreeHost(g->h_barrier_err);
   if (g->h_hdr) cudaFreeHost(g->h_hdr);
   if (g->h_scratch) cudaFreeHost(g->h_scratch);
+  if (g->h_kc_rec) cudaFreeHost(g->h_kc_rec);
   for (cudaEvent_t e : g->kt_events) cudaEventDestroy(e);
   if (g->ev_begin) cudaEventDestroy(g->ev_begin);
   if (g->ev_end) cudaEventDestroy(g->ev_end);

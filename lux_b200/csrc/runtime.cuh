@@ -9,6 +9,7 @@
 #include "push.cuh"
 #include "bc.cuh"
 #include "tc.cuh"
+#include "kcore.cuh"
 
 // fix-up scratch of one tiled sweep (pull.cuh): per-tile partials and carries, per-block aggregates
 struct FixupScratch {
@@ -193,6 +194,23 @@ struct luxb_graph {
   void* d_tc_sum_tmp = nullptr;
   size_t tc_sum_bytes = 0;
   int tc_group_grid = 0, tc_big_grid = 0;
+  // k-core decomposition (kcore.cuh): this rank's adjacency over all sources, the peel's state
+  uint64_t kc_m = 0;                  // undirected simple edges (2 kc_m adjacency entries over all ranks)
+  uint64_t* d_kc_off = nullptr;       // [nv + 1] offsets of every source's list of this rank's neighbours
+  uint32_t* d_kc_adj = nullptr;       // this rank's adjacency entries, targets in [row_left, row_right]
+  uint32_t* d_kc_deg0 = nullptr;      // [n_part] degrees
+  uint32_t* d_kc_deg = nullptr;       // [n_part] degrees during a run; check counters [2 n_part] after it
+  uint32_t* d_kc_core = nullptr;      // [nv] core numbers (the handle's values)
+  uint32_t* d_kc_alive[2] = {nullptr, nullptr};  // [n_part] alive lists
+  uint32_t* d_kc_piece[2] = {nullptr, nullptr};  // [n_part] this rank's pieces of F
+  uint32_t* d_kc_f = nullptr;         // [nv] the global F (several ranks)
+  uint64_t* d_kc_pre = nullptr;       // [nv + 1] slot offsets of F's lists
+  luxb::KcoreRec* d_kc_rec = nullptr;   // [1 + LUXB_MAX_PARTS] this rank's record, then every rank's
+  luxb::KcoreRec* h_kc_rec = nullptr;   // pinned host copy of the gathered records
+  unsigned long long* d_kc_bad = nullptr;
+  void* d_kc_scan_tmp = nullptr;
+  size_t kc_scan_bytes = 0;
+  int kc_grid = 0;                    // resident CTAs of the scatter and the tally
 
   // communication
   luxb::ncclComm_t comm = nullptr;

@@ -1,4 +1,4 @@
-"""PyTorch front-end of the C ABI (SURVEY §8 f4): the four Lux apps, weighted SSSP, betweenness centrality and triangle counting as `torch.ops.luxb.*` custom ops taking the CSC as
+"""PyTorch front-end of the C ABI (SURVEY §8 f4): the four Lux apps, weighted SSSP, betweenness centrality, triangle counting and k-core decomposition as `torch.ops.luxb.*` custom ops taking the CSC as
 torch tensors and returning torch tensors.  Plumbing only — every op opens a libluxb handle through the ctypes binding
 (lux_b200/binding.py), runs the app on the CUDA device of the current torch context and copies the result back; no torch
 kernel takes part in the computation, and there is no CPU fallback (the ops raise without a GPU).
@@ -12,6 +12,7 @@ kernel takes part in the computation, and there is no CPU fallback (the ops rais
     bc     = torch.ops.luxb.betweenness(row_end, src, sources)  # f64 [nv]  (Σ over sources of Brandes' δ, not normalised)
     bc     = torch.ops.luxb.betweenness_weighted(row_end, src, weight, sources)  # f64 [nv]  (weighted paths, weights >= 1)
     t      = torch.ops.luxb.triangles(row_end, src)             # i64 [nv]  (triangles at each vertex, undirected simple graph)
+    core   = torch.ops.luxb.core_number(row_end, src)           # i64 [nv]  (core number of each vertex, undirected simple graph)
 row_end: int64 [nv] END offsets (the .lux convention); src: int64/int32 [ne]; weight: int32 [ne]; sources: int64/int32 [k] vertex ids."""
 import numpy as np
 import torch
@@ -36,6 +37,7 @@ _lib.define("sssp_weighted(Tensor row_end, Tensor src, Tensor weight, int start)
 _lib.define("betweenness(Tensor row_end, Tensor src, Tensor sources) -> Tensor")
 _lib.define("betweenness_weighted(Tensor row_end, Tensor src, Tensor weight, Tensor sources) -> Tensor")
 _lib.define("triangles(Tensor row_end, Tensor src) -> Tensor")
+_lib.define("core_number(Tensor row_end, Tensor src) -> Tensor")
 
 
 def _pagerank(row_end, src, num_iter):
@@ -81,7 +83,12 @@ def _triangles(row_end, src):
     return torch.from_numpy(out["per_vertex"].astype(np.int64)).to(row_end.device)
 
 
+def _core_number(row_end, src):
+    out = _apps.core_number(_np(row_end, np.uint64), _np(src, np.uint32), device=_device_index(row_end))
+    return torch.from_numpy(out["core"].astype(np.int64)).to(row_end.device)
+
+
 for _name, _fn in (("pagerank", _pagerank), ("components", _components), ("sssp", _sssp), ("colfilter", _colfilter),
                    ("sssp_weighted", _sssp_weighted), ("betweenness", _betweenness), ("betweenness_weighted", _betweenness_weighted),
-                   ("triangles", _triangles)):
+                   ("triangles", _triangles), ("core_number", _core_number)):
     _lib.impl(_name, _fn, "CompositeExplicitAutograd")
