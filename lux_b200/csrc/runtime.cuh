@@ -74,6 +74,80 @@ struct PhaseTimer {
   long cnt = 0;
 };
 
+// col_filter (cf.cuh): the chunk table of this rank's destinations
+struct CfState {
+  uint32_t* chunk_first = nullptr;
+  uint32_t* chunk_vtx = nullptr;
+  uint32_t n_chunks = 0;
+  float* partial = nullptr;
+};
+
+// betweenness centrality (bc.cuh): the BFS of the label engine, then per source the level lists, σ and δ; scores summed
+// over sources
+struct BcState {
+  double* sigma = nullptr;       // [nv] path counts of the last source
+  double* delta = nullptr;       // [nv] dependencies of the last source
+  double* scores = nullptr;      // [nv] Σ δ over the sources processed (the handle's values)
+  uint32_t* order = nullptr;     // [nv] reached ids sorted stably by level (weighted: by distance)
+  double* lvl = nullptr;         // one level's sums, in level order (grown to the largest level seen)
+  uint64_t lvl_cap = 0;
+  uint32_t* off = nullptr;       // level_off[L + 1] (weighted: class_off, one entry per distinct distance)
+  uint64_t off_cap = 0;
+  uint32_t* split = nullptr;     // nranks > 1: [L][P + 1] every partition's piece of every level
+  uint64_t split_cap = 0;
+  void* sort_tmp = nullptr;
+  size_t sort_bytes = 0;
+  uint32_t* ctl = nullptr;       // [0..1] BcCtl of the level being summed, [2] deepest level (weighted: largest
+                                 // distance), [3] weighted: reached vertices, [4] weighted: class count
+  luxb::BcHub* hubs = nullptr;
+  double* partial = nullptr;
+  std::vector<uint32_t> h_off, h_split;  // host copies of this source's level_off / split
+  bool has_source = false;
+};
+
+// triangle counting (tc.cuh): the oriented adjacency of the whole graph and the bins of this rank's range
+struct TcState {
+  uint64_t m = 0;                  // undirected simple edges
+  uint64_t* off = nullptr;         // [nv + 1] out-list offsets
+  uint32_t* dst = nullptr;         // [m] out-lists N+(u), ascending ids
+  uint32_t* staged = nullptr;      // vertices of the grouped kernel
+  uint64_t* stage_pre = nullptr;
+  uint32_t* group = nullptr;
+  uint32_t* big = nullptr;         // vertices of the big kernel
+  uint32_t n_group = 0, n_big = 0;
+  unsigned long long* t = nullptr;      // [nv] per-vertex counts (the handle's values)
+  unsigned long long* total = nullptr;  // [1] sum of t
+  unsigned int* next = nullptr;         // [2] work counters
+  void* sum_tmp = nullptr;
+  size_t sum_bytes = 0;
+  int group_grid = 0, big_grid = 0;
+};
+
+// k-core decomposition (kcore.cuh): this rank's adjacency over all sources, the peel's state
+struct KcoreState {
+  uint64_t m = 0;                  // undirected simple edges (2 m adjacency entries over all ranks)
+  uint64_t* off = nullptr;         // [nv + 1] offsets of every source's list of this rank's neighbours
+  uint32_t* adj = nullptr;         // this rank's adjacency entries, targets in [row_left, row_right]
+  uint32_t* deg0 = nullptr;        // [n_part] degrees
+  uint32_t* deg = nullptr;         // [n_part] degrees during a run; check counters [2 n_part] after it
+  uint32_t* core = nullptr;        // [nv] core numbers (the handle's values)
+  uint32_t* alive[2] = {nullptr, nullptr};  // [n_part] alive lists
+  uint32_t* piece[2] = {nullptr, nullptr};  // [n_part] this rank's pieces of F
+  uint32_t* f = nullptr;           // [nv] the global F (several ranks)
+  uint64_t* pre = nullptr;         // [nv + 1] slot offsets of F's lists
+  luxb::KcoreRec* rec = nullptr;   // [1 + LUXB_MAX_PARTS] this rank's record, then every rank's
+  luxb::KcoreRec* h_rec = nullptr; // pinned host copy of the gathered records
+  unsigned long long* bad = nullptr;
+  void* scan_tmp = nullptr;
+  size_t scan_bytes = 0;
+  int grid = 0;                    // resident CTAs of the scatter and the tally
+};
+
+// one buffer the graph keeps: device memory, pinned host memory, or pinned host memory mapped into the device's
+// address space
+enum class MemKind : uint8_t { kDevice, kPinned, kMapped };
+struct OwnedBuf { void* p; MemKind kind; };
+
 struct luxb_graph {
   luxb_config cfg{};
   uint32_t nv = 0;
@@ -116,7 +190,6 @@ struct luxb_graph {
   uint32_t* d_deg = nullptr;   // PageRank: global out-degrees
   void* d_val[2] = {nullptr, nullptr};  // replicas of the vertex values (labels: only [0])
   int cur = 0;
-  size_t vbytes = 4;           // bytes per vertex value
   // hot-packed gather layout (PageRank): hot copies live in d_hot, natural-order values in d_val[0/1]
   uint32_t hot_n = 0;
   void* d_hot = nullptr;             // [hot_n] hot copies (single buffer: refreshed in place after every iteration)
@@ -155,62 +228,10 @@ struct luxb_graph {
   uint32_t* h_hdr = nullptr;          // pinned [2 * P]: type, count of the current frontier of every partition
   uint32_t* h_scratch = nullptr;      // pinned scratch (header readback)
   unsigned long long* d_counters = nullptr;  // [0] edges scanned by push kernels, [1] check mistakes
-  // col_filter
-  uint32_t* d_chunk_first = nullptr;
-  uint32_t* d_chunk_vtx = nullptr;
-  uint32_t n_chunks = 0;
-  float* d_partial = nullptr;
-  // betweenness centrality (bc.cuh): the BFS above, then per source the level lists, σ and δ; scores summed over sources
-  double* d_sigma = nullptr;       // [nv] path counts of the last source
-  double* d_delta = nullptr;       // [nv] dependencies of the last source
-  double* d_scores = nullptr;      // [nv] Σ δ over the sources processed (the handle's values)
-  uint32_t* d_order = nullptr;     // [nv] reached ids sorted stably by level (weighted: by distance)
-  double* d_bc_lvl = nullptr;      // one level's sums, in level order (grown to the largest level seen)
-  uint64_t bc_lvl_cap = 0;
-  uint32_t* d_bc_off = nullptr;    // level_off[L + 1] (weighted: class_off, one entry per distinct distance)
-  uint64_t bc_off_cap = 0;
-  uint32_t* d_bc_split = nullptr;  // nranks > 1: [L][P + 1] every partition's piece of every level
-  uint64_t bc_split_cap = 0;
-  void* d_bc_sort_tmp = nullptr;
-  size_t bc_sort_bytes = 0;
-  uint32_t* d_bc_ctl = nullptr;    // [0..1] BcCtl of the level being summed, [2] deepest level (weighted: largest
-                                   // distance), [3] weighted: reached vertices, [4] weighted: class count
-  luxb::BcHub* d_bc_hubs = nullptr;
-  double* d_bc_partial = nullptr;
-  std::vector<uint32_t> bc_off, bc_split;  // host copies of this source's level_off / split
-  bool bc_has_source = false;
-  // triangle counting (tc.cuh): the oriented adjacency of the whole graph and the bins of this rank's range
-  uint64_t tc_m = 0;               // undirected simple edges
-  uint64_t* d_tc_off = nullptr;    // [nv + 1] out-list offsets
-  uint32_t* d_tc_dst = nullptr;    // [tc_m] out-lists N+(u), ascending ids
-  uint32_t* d_tc_staged = nullptr; // vertices of the grouped kernel
-  uint64_t* d_tc_stage_pre = nullptr;
-  uint32_t* d_tc_group = nullptr;
-  uint32_t* d_tc_big = nullptr;    // vertices of the big kernel
-  uint32_t tc_n_group = 0, tc_n_big = 0;
-  unsigned long long* d_tc_t = nullptr;  // [nv] per-vertex counts (the handle's values)
-  unsigned long long* d_tc_total = nullptr;  // [1] sum of t
-  unsigned int* d_tc_next = nullptr;         // [2] work counters
-  void* d_tc_sum_tmp = nullptr;
-  size_t tc_sum_bytes = 0;
-  int tc_group_grid = 0, tc_big_grid = 0;
-  // k-core decomposition (kcore.cuh): this rank's adjacency over all sources, the peel's state
-  uint64_t kc_m = 0;                  // undirected simple edges (2 kc_m adjacency entries over all ranks)
-  uint64_t* d_kc_off = nullptr;       // [nv + 1] offsets of every source's list of this rank's neighbours
-  uint32_t* d_kc_adj = nullptr;       // this rank's adjacency entries, targets in [row_left, row_right]
-  uint32_t* d_kc_deg0 = nullptr;      // [n_part] degrees
-  uint32_t* d_kc_deg = nullptr;       // [n_part] degrees during a run; check counters [2 n_part] after it
-  uint32_t* d_kc_core = nullptr;      // [nv] core numbers (the handle's values)
-  uint32_t* d_kc_alive[2] = {nullptr, nullptr};  // [n_part] alive lists
-  uint32_t* d_kc_piece[2] = {nullptr, nullptr};  // [n_part] this rank's pieces of F
-  uint32_t* d_kc_f = nullptr;         // [nv] the global F (several ranks)
-  uint64_t* d_kc_pre = nullptr;       // [nv + 1] slot offsets of F's lists
-  luxb::KcoreRec* d_kc_rec = nullptr;   // [1 + LUXB_MAX_PARTS] this rank's record, then every rank's
-  luxb::KcoreRec* h_kc_rec = nullptr;   // pinned host copy of the gathered records
-  unsigned long long* d_kc_bad = nullptr;
-  void* d_kc_scan_tmp = nullptr;
-  size_t kc_scan_bytes = 0;
-  int kc_grid = 0;                    // resident CTAs of the scatter and the tally
+  CfState cf;
+  BcState bc;
+  TcState tc;
+  KcoreState kc;
 
   // communication
   luxb::ncclComm_t comm = nullptr;
@@ -261,7 +282,7 @@ struct luxb_graph {
   std::vector<cudaEvent_t> kt_events;  // pairs
   size_t kt_used = 0;
 
-  std::vector<void*> host_allocs;  // edge arrays living in mapped pinned host memory (cfg.zero_copy_edges)
+  std::vector<OwnedBuf> owned;  // every buffer above, in order of allocation (api.cu: gmalloc); luxb_close frees them
 
   // stats / trace
   luxb_stats_t stats{};
