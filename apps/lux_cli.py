@@ -11,6 +11,7 @@
                                                                                    # weighted BC (i32 trailer, w >= 1; ours)
   python apps/lux_cli.py tc         -ng 1 -file g.lux [-out t.npy]                  # triangle counting (ours)
   python apps/lux_cli.py kcore      -ng 1 -file g.lux [-check] [-out core.npy]      # k-core decomposition (ours)
+  python apps/lux_cli.py truss      -ng 1 -file g.lux [-check] [-out truss.npz]     # k-truss decomposition (ours)
   python apps/lux_cli.py converter  -nv N -ne M -input edges.txt -output g.lux     # tools/converter.cc:13-39 (host only)
 
 `-ll:gpu N` is accepted as a synonym of `-ng N` (README.md:47); -ll:fsize / -ll:zsize are accepted and ignored (HBM is
@@ -34,6 +35,12 @@ and "TRIANGLES = T" on rank 0, and no "[Memory Setting]" line; `-out` saves the 
 prints "ELAPSED TIME" (device time of the peel) and "DEGENERACY = K" (the largest core number) on rank 0, and no
 "[Memory Setting]" line; `-check` prints the check line above per rank (vertices that are not a fixpoint of the h-index
 operator); `-out` saves the u32 core numbers.
+
+`truss` (no reference counterpart) computes the support and truss number of every edge of the same undirected simple
+graph.  It prints "ELAPSED TIME" (device time of the support count and the peel) and "KMAX = K" (the largest truss
+number) on rank 0, and no "[Memory Setting]" line; `-check` prints the check line above per rank (this rank's edges that
+fail the truss check); `-out` saves an .npz with the u32 arrays lo, hi (the edges, ascending), support, truss and vertex
+(the largest truss number at each vertex).
 """
 import os
 import subprocess
@@ -44,7 +51,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-APPS = {"pagerank": 0, "components": 1, "sssp": 2, "colfilter": 3, "bc": 5, "tc": 7, "kcore": 8}
+APPS = {"pagerank": 0, "components": 1, "sssp": 2, "colfilter": 3, "bc": 5, "tc": 7, "kcore": 8, "truss": 9}
 
 
 def parse(argv):
@@ -166,7 +173,7 @@ def main():
     g = L.LuxGraph.from_file(opt["file"], app=weighted_app[app] if weighted else APPS[app], rank=rank, nranks=world, device=local,
                              start=opt["start"], verbose=opt["verbose"])
     b = g.bounds()
-    if rank == 0 and app not in ("bc", "tc", "kcore"):
+    if rank == 0 and app not in ("bc", "tc", "kcore", "truss"):
         fb, zc = memory_setting(app, g.nv, g.ne, b, int(b["fq_right"][-1]) + 1, weighted)
         print("[Memory Setting] Set ll:fsize >= %dMB and ll:zsize >= %dMB" % (fb, zc), flush=True)
     g.comm_init_torch()
@@ -179,6 +186,8 @@ def main():
         total = g.tc_run()
     elif app == "kcore":
         degeneracy = g.kcore_run()
+    elif app == "truss":
+        kmax = g.truss_run()
     else:
         g.run_to_convergence()
     if rank == 0:
@@ -187,13 +196,18 @@ def main():
             print("TRIANGLES = %d" % total, flush=True)
         if app == "kcore":
             print("DEGENERACY = %d" % degeneracy, flush=True)
-    if opt["check"] and app in ("components", "sssp", "kcore"):
+        if app == "truss":
+            print("KMAX = %d" % kmax, flush=True)
+    if opt["check"] and app in ("components", "sssp", "kcore", "truss"):
         bad = g.check()
         print("[%s] Check task: rowLeft(%u) numMistakes(%u)" % ("PASS" if bad == 0 else "FAIL", int(b["row_left"][rank]), bad),
               flush=True)
     if opt["out"]:
         vals = g.values()
-        if rank == 0:
+        if rank == 0 and app == "truss":
+            lo, hi, support, truss = g.truss_edges()
+            np.savez(opt["out"], lo=lo, hi=hi, support=support, truss=truss, vertex=vals)
+        elif rank == 0:
             np.save(opt["out"], vals)
     g.close()
     if world > 1:

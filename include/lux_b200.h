@@ -56,8 +56,11 @@ typedef enum {
                             distances (weights >= 1), f64 score per vertex; runs through luxb_bc_run */
   LUXB_TC = 7,           /* triangle counting (no reference counterpart) — exact u64 count of the triangles at every
                             vertex of the undirected simple graph; runs through luxb_tc_run */
-  LUXB_KCORE = 8         /* k-core decomposition (no reference counterpart) — exact u32 core number of every vertex of
+  LUXB_KCORE = 8,        /* k-core decomposition (no reference counterpart) — exact u32 core number of every vertex of
                             the undirected simple graph, by level-synchronous peeling; runs through luxb_kcore_run */
+  LUXB_TRUSS = 9         /* k-truss decomposition (no reference counterpart) — exact u32 support and truss number of every
+                            edge of the undirected simple graph, by level-synchronous edge peeling; runs through
+                            luxb_truss_run */
 } luxb_app;
 
 /* Weighted SSSP (LUXB_SSSP_WEIGHTED):
@@ -147,6 +150,35 @@ typedef enum {
  * same figure on every rank), loop_seconds = device time of the run.  luxb_trace holds the last run, one entry per
  * round: active = |F| over all ranks, pull = that round's k.  cfg.start_vtx, cfg.exchange, cfg.verbose and
  * cfg.balanced_split have no effect: the work split is the reference's (luxb_work_bounds says so). */
+
+/* k-truss decomposition (LUXB_TRUSS).  The graph is LUXB_TC's: {u, v} is an edge iff u != v and u -> v or v -> u is
+ * stored (parallel edges, both directions and self-loops collapse; weights are ignored, a weighted CSC is accepted).  m is
+ * the number of undirected edges; edge ids are u32, the rank of (lo, hi), lo < hi, in ascending order.  A graph with
+ * m >= 2^32 fails luxb_init with LUXB_ERR_ARG.
+ *  - sup(e) for e = {u, v} is |N(u) ∩ N(v)|, the number of triangles that contain e.
+ *  - τ(e) (u32) is the largest k >= 2 such that e lies in a subgraph in which every edge is in at least k - 2 triangles
+ *    of that subgraph: the edges with τ >= k are exactly those of networkx's k_truss(G, k), for every k.
+ *  - The vertex truss tv(v) is the largest τ over the edges at v, 0 for a vertex without edges: v is a vertex of
+ *    k_truss(G, k) iff tv(v) >= k.  kmax is the largest τ: 0 without edges, 2 with edges but no triangle.
+ *  - The peel, with ℓ = k - 2: ℓ = 0; while an edge is alive: ℓ = max(ℓ, min sup over the alive edges); repeat:
+ *    F = {alive e : sup(e) <= ℓ}, stop if F is empty; τ[F] = ℓ + 2; every triangle whose three edges were all alive when
+ *    the round started and which has an edge in F lowers the support of each of its edges not in F by exactly one (the F
+ *    edge of the smallest id applies it); remove F.  A round is one non-empty F, a level one value of ℓ with at least one
+ *    round.  Every decrement lands on an edge whose support still counts that triangle, so no support goes below zero
+ *    and the rounds' sets do not depend on the schedule or on the number of ranks.
+ * luxb_init builds, on every rank, the edge table, the oriented lists of triangle counting and the symmetric adjacency
+ * with an edge id per entry, and counts the support.  The handle's values (luxb_get_values / luxb_get_local_values) are
+ * tv, 4 bytes per vertex: zeros before the first luxb_truss_run, complete on every rank after one.  luxb_set_values /
+ * luxb_set_local_values, luxb_iterate and luxb_run_to_convergence return LUXB_ERR_ARG; luxb_truss_set_truss overwrites τ
+ * instead, so that luxb_check can judge any assignment.
+ * luxb_check counts this rank's edges (an edge {lo, hi} belongs to the rank whose work range holds lo) that fail the
+ * check: with c = τ(e), a = |{w in N(u) ∩ N(v) : min(τ(u, w), τ(v, w)) >= c}| and b the same count with >= c + 1, e is a
+ * violation iff c < 2, a < c - 2 or b >= c - 1.  True truss numbers always pass: e lies in the c-truss, so a >= c - 2;
+ * and if b >= c - 1, the (c + 1)-truss together with e would have every support >= c - 1, which puts e in the
+ * (c + 1)-truss.  Passing is necessary, not sufficient: all 2s pass.
+ * luxb_stats: iterations += rounds, edges_processed += m per run, loop_seconds = device time of the run (support and
+ * peel).  luxb_trace holds the last run, one entry per round: active = |F| over all ranks, pull = that round's k.
+ * cfg.start_vtx, cfg.exchange, cfg.verbose and cfg.balanced_split have no effect. */
 
 typedef enum {
   LUXB_EXCHANGE_NCCL = 0, /* library collectives only: PageRank packs its share and broadcasts the two ranges of every
@@ -266,7 +298,7 @@ int luxb_iterate(luxb_graph* g, int iters, uint64_t* active_out);
 int luxb_run_to_convergence(luxb_graph* g, int max_iters, int* iters_out);
 
 /* ---- results / check / stats -------------------------------------------------------------------------------- */
-/* Full vertex-value array (what the reference holds in dist_lr[iter%2]): nv * {4 | 4 | 80 | 8 (BC scores, TC counts) | 4 (core numbers)} bytes.  PageRank on
+/* Full vertex-value array (what the reference holds in dist_lr[iter%2]): nv * {4 | 4 | 80 | 8 (BC scores, TC counts) | 4 (core numbers, vertex truss)} bytes.  PageRank on
  * nranks > 1 exchanges only the values that are ever gathered each iteration and completes the full array on demand:
  * there the call is collective (every rank calls it at the same point). */
 int luxb_get_values(luxb_graph* g, void* host_out, size_t bytes);
@@ -350,6 +382,22 @@ int luxb_tc_run(luxb_graph* g, uint64_t* total_out);
  * NULL).  Collective on nranks > 1: each rank peels its own range, the pieces of every round's F are exchanged, and the
  * core numbers are completed on every rank at the end.  LUXB_ERR_STATE before luxb_init, LUXB_ERR_ARG on another app. */
 int luxb_kcore_run(luxb_graph* g, uint32_t* degeneracy_out);
+
+/* ---- k-truss decomposition (LUXB_TRUSS handles) ------------------------------------------------------------------- */
+/* Recompute the support and every truss number from scratch and write kmax to *kmax_out (may be NULL).  Collective on
+ * nranks > 1: each rank counts the support at its own range and the supports are summed; every rank then walks the whole
+ * of every round's F but lowers only its own edges, and only F moves between the ranks.  LUXB_ERR_STATE before luxb_init
+ * (and if the schedule's invariant breaks), LUXB_ERR_ARG on another app. */
+int luxb_truss_run(luxb_graph* g, uint32_t* kmax_out);
+/* m, the number of undirected simple edges. */
+int luxb_truss_num_edges(const luxb_graph* g, uint64_t* m_out);
+/* Every edge in ascending (lo, hi) order, lo < hi, with its support in the input graph and τ (zero before the first
+ * run); a NULL pointer skips that array, m other than the graph's is LUXB_ERR_ARG.  Every rank holds all of it: not
+ * collective. */
+int luxb_truss_edges(luxb_graph* g, luxb_vid* lo, luxb_vid* hi, uint32_t* support, uint32_t* truss, uint64_t m);
+/* Overwrite τ (m entries, edge order as above) so that luxb_check can judge any assignment; tv follows.  The next
+ * luxb_truss_run recomputes τ. */
+int luxb_truss_set_truss(luxb_graph* g, const uint32_t* truss, uint64_t m);
 
 void luxb_close(luxb_graph* g);
 const char* luxb_last_error(void);

@@ -8,11 +8,12 @@ betweenness: Brandes from a list of sources over the SSSP engine's hop levels, o
              SSSP distances (ours; the reference has no BC)
 triangles  : exact triangle counts of the undirected simple graph (ours)
 core_number: exact core numbers of the undirected simple graph, by level-synchronous peeling (ours)
+truss      : exact edge support and truss numbers of the undirected simple graph, by level-synchronous edge peeling (ours)
 Single-rank convenience wrappers; multi-GPU callers drive LuxGraph directly (see bench.py).
 """
 import numpy as np
 
-from .binding import LuxGraph, APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC, APP_BC_WEIGHTED, APP_TC, APP_KCORE
+from .binding import LuxGraph, APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC, APP_BC_WEIGHTED, APP_TC, APP_KCORE, APP_TRUSS
 
 
 def pagerank(row_end, src, num_iter=10, device=0):
@@ -85,3 +86,15 @@ def core_number(row_end, src, device=0):
         g.init()
         degeneracy = g.kcore_run()
         return dict(core=g.values(), degeneracy=degeneracy, rounds=g.stats()["iterations"])
+
+
+def truss(row_end, src, device=0):
+    """k-truss decomposition of the CSC read as an undirected simple graph ({u, v} is an edge iff u != v and u -> v or
+    v -> u is stored; weights are ignored): dict(lo, hi = u32 [m] the edges in ascending (lo, hi) order, support = u32 [m]
+    triangles at each edge, truss = u32 [m] truss numbers (the edges with truss >= k are networkx's k_truss(G, k)),
+    vertex = u32 [nv] the largest truss number at each vertex, kmax, rounds = the peel's rounds)."""
+    with LuxGraph.from_csc(row_end, src, app=APP_TRUSS, device=device) as g:
+        g.init()
+        kmax = g.truss_run()
+        lo, hi, support, tr = g.truss_edges()
+        return dict(lo=lo, hi=hi, support=support, truss=tr, vertex=g.values(), kmax=kmax, rounds=g.stats()["iterations"])

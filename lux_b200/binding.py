@@ -6,7 +6,7 @@ import numpy as np
 
 from . import build as _build
 
-APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC, APP_BC_WEIGHTED, APP_TC, APP_KCORE = 0, 1, 2, 3, 4, 5, 6, 7, 8
+APP_PAGERANK, APP_CC, APP_SSSP, APP_COLFILTER, APP_SSSP_WEIGHTED, APP_BC, APP_BC_WEIGHTED, APP_TC, APP_KCORE, APP_TRUSS = 0, 1, 2, 3, 4, 5, 6, 7, 8, 9
 DIST_INF = 0xFFFFFFFF  # APP_SSSP_WEIGHTED / APP_BC_WEIGHTED: distance of an unreachable vertex (LUXB_DIST_INF)
 EXCHANGE_NCCL, EXCHANGE_P2P, EXCHANGE_P2P_FUSED = 0, 1, 2
 DENSE_BITMAP, SPARSE_QUEUE = 0x1234567, 0x7654321
@@ -121,7 +121,7 @@ def convert_edgelist(edge_list_path, lux_path, nv, ne):
 
 _VDTYPE = {APP_PAGERANK: np.float32, APP_CC: np.uint32, APP_SSSP: np.uint32, APP_COLFILTER: np.float32,
            APP_SSSP_WEIGHTED: np.uint32, APP_BC: np.float64, APP_BC_WEIGHTED: np.float64,
-           APP_TC: np.uint64, APP_KCORE: np.uint32}
+           APP_TC: np.uint64, APP_KCORE: np.uint32, APP_TRUSS: np.uint32}
 
 
 class LuxGraph:
@@ -343,6 +343,32 @@ class LuxGraph:
         degeneracy = C.c_uint32(0)
         _chk(load_library().luxb_kcore_run(self._h, C.byref(degeneracy)), "luxb_kcore_run")
         return degeneracy.value
+
+    def truss_run(self):
+        """k-truss decomposition (APP_TRUSS handles): recompute the support and truss number of every edge of the
+        undirected simple graph (values() returns the vertex truss, the largest truss number at each vertex) and return
+        kmax.  Collective on nranks > 1."""
+        kmax = C.c_uint32(0)
+        _chk(load_library().luxb_truss_run(self._h, C.byref(kmax)), "luxb_truss_run")
+        return kmax.value
+
+    def truss_num_edges(self):
+        m = C.c_uint64(0)
+        _chk(load_library().luxb_truss_num_edges(self._h, C.byref(m)), "luxb_truss_num_edges")
+        return m.value
+
+    def truss_edges(self):
+        """(lo, hi, support, truss), u32 [m] each, edges in ascending (lo, hi) order with lo < hi; support of the input
+        graph, truss numbers of the last run (zeros before the first)."""
+        m = self.truss_num_edges()
+        lo, hi, sup, tr = (np.empty(m, np.uint32) for _ in range(4))
+        _chk(load_library().luxb_truss_edges(self._h, _p(lo), _p(hi), _p(sup), _p(tr), C.c_uint64(m)), "luxb_truss_edges")
+        return lo, hi, sup, tr
+
+    def set_truss(self, truss):
+        """Overwrite the truss numbers (u32 [m], the order of truss_edges()) so that check() judges them."""
+        t = np.ascontiguousarray(truss, np.uint32)
+        _chk(load_library().luxb_truss_set_truss(self._h, _p(t) if t.size else None, C.c_uint64(t.size)), "luxb_truss_set_truss")
 
     def enable_kernel_timing(self, on=True):
         _chk(load_library().luxb_enable_kernel_timing(self._h, C.c_int(1 if on else 0)), "luxb_enable_kernel_timing")

@@ -48,9 +48,10 @@ static constexpr AppInfo kApps[] = {
     {"weighted betweenness centrality", AppRun::kEntry,       kBcRun,           true,   true,  8,        false, true},
     {"triangle counting",               AppRun::kEntry,       "luxb_tc_run",    false,  false, 8,        false, false},
     {"k-core decomposition",            AppRun::kEntry,       "luxb_kcore_run", false,  false, 4,        true,  true},
+    {"k-truss decomposition",           AppRun::kEntry,       "luxb_truss_run", false,  false, 4,        true,  false},
 };
 static constexpr int kNumApps = sizeof(kApps) / sizeof(kApps[0]);
-static_assert(kNumApps == LUXB_KCORE + 1, "one row per luxb_app");
+static_assert(kNumApps == LUXB_TRUSS + 1, "one row per luxb_app");
 // the handle's app (its config passed check_config at open)
 static const AppInfo& app_of(const luxb_graph* g) { return kApps[g->cfg.app]; }
 
@@ -1162,6 +1163,7 @@ static int wait_cold_exchange(luxb_graph* g);
 static int bc_alloc(luxb_graph* g);
 static int tc_build(luxb_graph* g);
 static int kcore_build(luxb_graph* g);
+static int truss_build(luxb_graph* g);
 
 // The gather side of the pull sweeps: global out-degrees, the hot set (build_hot_layout), the flagged streams if
 // `streams` (build_seg_sweep) and the hot copies Z = [hot | compact cold values on one rank] + one whole table of slack:
@@ -1268,6 +1270,7 @@ int luxb_init(luxb_graph* g) {
     }
     case LUXB_TC: LUXB_TRY(tc_build(g)); break;
     case LUXB_KCORE: LUXB_TRY(kcore_build(g)); break;
+    case LUXB_TRUSS: LUXB_TRY(truss_build(g)); break;
   }
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
   g->cur = 0;
@@ -2801,7 +2804,7 @@ static int tc_sort_unique(luxb_graph* g, DevTmp& tmp, uint64_t* keys, uint64_t* 
 
 // The distinct undirected keys min << 32 | max of the whole graph, on every rank (on several ranks every rank's distinct
 // keys go to every rank), at the front of *keys; *alt is a buffer of the same size.  Both belong to `tmp`.  The graph of
-// LUXB_TC and LUXB_KCORE.
+// LUXB_TC, LUXB_KCORE and LUXB_TRUSS.
 static int undirected_keys(luxb_graph* g, DevTmp& tmp, int bits, uint64_t** keys_out, uint64_t** alt_out, uint64_t* m_out) {
   const int grid = g->num_sms * 8;
   uint64_t *d_keys = nullptr, *d_alt = nullptr;
@@ -2859,17 +2862,12 @@ static int pair_key_bits(uint32_t nv) {
   return 32 + vbits;
 }
 
-// luxb_init of a LUXB_TC handle: the undirected simple edges of the whole graph (undirected_keys), the oriented
-// out-lists, the work per vertex and the bins of this rank's range
-static int tc_build(luxb_graph* g) {
-  DevTmp tmp;
+// The oriented out-lists of the m undirected keys (oriented in place, then released with `alt`), the work per vertex
+// and the bins of this rank's range, into `tc` (off, dst, staged, stage_pre, group, n_group, big, n_big).  LUXB_TC and
+// LUXB_TRUSS.
+static int tc_orient_bins(luxb_graph* g, DevTmp& tmp, int bits, uint64_t* d_keys, uint64_t* d_alt, uint64_t m, TcState& tc) {
   const int grid = g->num_sms * 8;
   const uint32_t nv = g->nv;
-  const int bits = pair_key_bits(nv);  // min < nv in the high word, max in the low one
-  uint64_t *d_keys = nullptr, *d_alt = nullptr;
-  uint64_t m = 0;
-  LUXB_TRY(undirected_keys(g, tmp, bits, &d_keys, &d_alt, &m));
-  g->tc.m = m;
   // degrees, orientation, out-lists sorted by (from, to), offsets and the work W(u)
   uint32_t *d_deg = nullptr, *d_outdeg = nullptr;
   unsigned long long* d_work = nullptr;
@@ -2890,59 +2888,73 @@ static int tc_build(luxb_graph* g) {
     }));
     d_sorted = db.Current();
   }
-  LUXB_TRY(gmalloc(g, &g->tc.off, (uint64_t)nv + 1));
-  LUXB_CUDA(cudaMemsetAsync(g->tc.off + nv, 0, 8, g->stream));
-  widen_u32_to_u64_kernel<<<grid_for(nv, 256, grid), 256, 0, g->stream>>>(d_outdeg, g->tc.off, nv);
+  LUXB_TRY(gmalloc(g, &tc.off, (uint64_t)nv + 1));
+  LUXB_CUDA(cudaMemsetAsync(tc.off + nv, 0, 8, g->stream));
+  widen_u32_to_u64_kernel<<<grid_for(nv, 256, grid), 256, 0, g->stream>>>(d_outdeg, tc.off, nv);
   LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
-    return cub::DeviceScan::ExclusiveSum(t, b, g->tc.off, g->tc.off, (long long)nv + 1, g->stream);
+    return cub::DeviceScan::ExclusiveSum(t, b, tc.off, tc.off, (long long)nv + 1, g->stream);
   }));
-  LUXB_TRY(gmalloc(g, &g->tc.dst, m + 8));
-  if (m) tc_lists_kernel<<<grid_for(m, 256, grid), 256, 0, g->stream>>>(d_sorted, m, g->tc.off, g->tc.dst, d_work);
+  LUXB_TRY(gmalloc(g, &tc.dst, m + 8));
+  if (m) tc_lists_kernel<<<grid_for(m, 256, grid), 256, 0, g->stream>>>(d_sorted, m, tc.off, tc.dst, d_work);
   LUXB_CUDA(cudaGetLastError());
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
   for (void* q : {(void*)d_keys, (void*)d_alt, (void*)d_deg, (void*)d_outdeg}) tmp.release(q);
   // bins of this rank's range: staged vertices (grouped kernel) and big ones
   uint32_t* d_sel = nullptr;
   LUXB_TRY(tmp.alloc(&d_sel, 2));
-  LUXB_TRY(gmalloc(g, &g->tc.staged, g->n_part));
-  LUXB_TRY(gmalloc(g, &g->tc.big, g->n_part));
+  LUXB_TRY(gmalloc(g, &tc.staged, g->n_part));
+  LUXB_TRY(gmalloc(g, &tc.big, g->n_part));
   uint32_t n_sel[2] = {0, 0};
   if (g->n_part) {
     thrust::counting_iterator<uint32_t> ids(g->row_left);
     LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
-      return cub::DeviceSelect::If(t, b, ids, g->tc.staged, d_sel, (int)g->n_part, TcStaged{g->tc.off}, g->stream);
+      return cub::DeviceSelect::If(t, b, ids, tc.staged, d_sel, (int)g->n_part, TcStaged{tc.off}, g->stream);
     }));
     LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
-      return cub::DeviceSelect::If(t, b, ids, g->tc.big, d_sel + 1, (int)g->n_part, TcBig{g->tc.off}, g->stream);
+      return cub::DeviceSelect::If(t, b, ids, tc.big, d_sel + 1, (int)g->n_part, TcBig{tc.off}, g->stream);
     }));
     LUXB_CUDA(cudaMemcpyAsync(n_sel, d_sel, 8, cudaMemcpyDeviceToHost, g->stream));
     LUXB_CUDA(cudaStreamSynchronize(g->stream));
   }
   const uint32_t n_staged = n_sel[0];
-  g->tc.n_big = n_sel[1];
+  tc.n_big = n_sel[1];
   // groups: exclusive prefixes of the staged list lengths and costs, a head wherever either crosses its multiple
   uint64_t* d_cost = nullptr;
   LUXB_TRY(tmp.alloc(&d_cost, (uint64_t)n_staged + 1));
-  LUXB_TRY(gmalloc(g, &g->tc.stage_pre, (uint64_t)n_staged + 1));
-  tc_cost_kernel<<<grid_for((uint64_t)n_staged + 1, 256, grid), 256, 0, g->stream>>>(g->tc.staged, n_staged, g->tc.off, d_work,
-                                                                                    g->tc.stage_pre, d_cost);
+  LUXB_TRY(gmalloc(g, &tc.stage_pre, (uint64_t)n_staged + 1));
+  tc_cost_kernel<<<grid_for((uint64_t)n_staged + 1, 256, grid), 256, 0, g->stream>>>(tc.staged, n_staged, tc.off, d_work,
+                                                                                    tc.stage_pre, d_cost);
   LUXB_CUDA(cudaGetLastError());
-  for (uint64_t* p : {g->tc.stage_pre, d_cost})
+  for (uint64_t* p : {tc.stage_pre, d_cost})
     LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
       return cub::DeviceScan::ExclusiveSum(t, b, p, p, (long long)n_staged + 1, g->stream);
     }));
-  LUXB_TRY(gmalloc(g, &g->tc.group, (uint64_t)n_staged + 1));
+  LUXB_TRY(gmalloc(g, &tc.group, (uint64_t)n_staged + 1));
   uint32_t n_group = 0;
   if (n_staged) {
     LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
-      return cub::DeviceSelect::If(t, b, thrust::counting_iterator<uint32_t>(0), g->tc.group, d_sel, (int)n_staged,
-                                   TcGroupHead{g->tc.stage_pre, d_cost}, g->stream);
+      return cub::DeviceSelect::If(t, b, thrust::counting_iterator<uint32_t>(0), tc.group, d_sel, (int)n_staged,
+                                   TcGroupHead{tc.stage_pre, d_cost}, g->stream);
     }));
     LUXB_CUDA(cudaMemcpyAsync(&n_group, d_sel, 4, cudaMemcpyDeviceToHost, g->stream));
     LUXB_CUDA(cudaStreamSynchronize(g->stream));
   }
-  LUXB_CUDA(cudaMemcpyAsync(g->tc.group + n_group, &n_staged, 4, cudaMemcpyHostToDevice, g->stream));
-  g->tc.n_group = n_group;
+  LUXB_CUDA(cudaMemcpyAsync(tc.group + n_group, &n_staged, 4, cudaMemcpyHostToDevice, g->stream));
+  tc.n_group = n_group;
+  return 0;
+}
+
+// luxb_init of a LUXB_TC handle: the undirected simple edges of the whole graph (undirected_keys), the oriented
+// out-lists, the work per vertex and the bins of this rank's range (tc_orient_bins)
+static int tc_build(luxb_graph* g) {
+  DevTmp tmp;
+  const uint32_t nv = g->nv;
+  const int bits = pair_key_bits(nv);  // min < nv in the high word, max in the low one
+  uint64_t *d_keys = nullptr, *d_alt = nullptr;
+  uint64_t m = 0;
+  LUXB_TRY(undirected_keys(g, tmp, bits, &d_keys, &d_alt, &m));
+  g->tc.m = m;
+  LUXB_TRY(tc_orient_bins(g, tmp, bits, d_keys, d_alt, m, g->tc));
   // the run's state: t, its sum, the work counters; a grid of resident CTAs per kernel
   LUXB_TRY(gmalloc(g, &g->tc.t, nv));
   LUXB_CUDA(cudaMemsetAsync(g->tc.t, 0, (size_t)nv * 8, g->stream));
@@ -3181,12 +3193,292 @@ static int kcore_check(luxb_graph* g, uint64_t* mistakes_out) {
   return 0;
 }
 
+// ---- k-truss decomposition (truss.cuh) ------------------------------------------------------------------------------
+// sup0 from scratch: TC's kernels with the edge sink over this rank's bins, summed over the ranks
+static int truss_support(luxb_graph* g) {
+  TrussState& t = g->tr;
+  LUXB_CUDA(cudaMemsetAsync(t.sup0, 0, (size_t)t.m * 4, g->stream));
+  LUXB_CUDA(cudaMemsetAsync(t.o.next, 0, 8, g->stream));
+  const TcArgs a{t.o.off, t.o.dst, t.o.staged, t.o.stage_pre, t.o.group, t.o.n_group, t.o.big, t.o.n_big, nullptr, t.o.next};
+  if (t.o.n_group) {
+    truss_support_group_kernel<<<(int)std::min<uint32_t>(t.o.n_group, t.group_grid), kTcThreads, 0, g->stream>>>(a, t.sup0, t.oid);
+    g->stats.kernel_launches++;
+  }
+  if (t.o.n_big) {
+    truss_support_big_kernel<<<(int)std::min<uint32_t>(t.o.n_big, t.big_grid), kTcThreads, 0, g->stream>>>(a, t.sup0, t.oid);
+    g->stats.kernel_launches++;
+  }
+  LUXB_CUDA(cudaGetLastError());
+  if (g->P > 1 && t.m) LUXB_NCCL(nccl().AllReduce(t.sup0, t.sup0, t.m, ncclUint32, ncclSum, g->comm, g->stream));
+  return 0;
+}
+
+// tv[v] = max τ over the edges at v
+static int truss_vertex_values(luxb_graph* g) {
+  TrussState& t = g->tr;
+  LUXB_CUDA(cudaMemsetAsync(t.tv, 0, (size_t)g->nv * 4, g->stream));
+  if (t.m) truss_vertex_kernel<<<grid_for(t.m, 256, g->num_sms * 8), 256, 0, g->stream>>>(t.ekey, t.m, t.truss, t.tv);
+  LUXB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// luxb_init of a LUXB_TRUSS handle: the undirected keys (undirected_keys) kept as the edge table, TC's oriented lists and
+// bins (tc_orient_bins) with the edge id of every oriented position, the symmetric adjacency with edge ids, the support
+static int truss_build(luxb_graph* g) {
+  DevTmp tmp;
+  TrussState& t = g->tr;
+  const int grid = g->num_sms * 8;
+  const uint32_t nv = g->nv;
+  const int bits = pair_key_bits(nv);
+  uint64_t *d_keys = nullptr, *d_alt = nullptr, m = 0;
+  LUXB_TRY(undirected_keys(g, tmp, bits, &d_keys, &d_alt, &m));
+  LUXB_ARG(m < (1ull << 32), "k-truss: %llu undirected edges, but edge ids are u32", (unsigned long long)m);
+  t.m = m;
+  LUXB_TRY(gmalloc(g, &t.ekey, m));
+  if (m) LUXB_CUDA(cudaMemcpyAsync(t.ekey, d_keys, m * 8, cudaMemcpyDeviceToDevice, g->stream));
+  uint64_t* d_range = nullptr;
+  LUXB_TRY(tmp.alloc(&d_range, 2));
+  truss_range_kernel<<<1, 32, 0, g->stream>>>(t.ekey, m, g->row_left, g->n_part, d_range);
+  LUXB_CUDA(cudaGetLastError());
+  uint64_t range[2] = {0, 0};
+  LUXB_CUDA(cudaMemcpyAsync(range, d_range, 16, cudaMemcpyDeviceToHost, g->stream));
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  t.e_lo = (uint32_t)range[0];
+  t.e_hi = (uint32_t)range[1];
+  LUXB_TRY(tc_orient_bins(g, tmp, bits, d_keys, d_alt, m, t.o));  // orients and releases d_keys / d_alt
+  LUXB_TRY(gmalloc(g, &t.oid, m));
+  if (m) truss_orient_ids_kernel<<<grid, 256, 0, g->stream>>>(t.o.off, t.o.dst, nv, t.ekey, m, t.oid);
+  LUXB_CUDA(cudaGetLastError());
+  // the symmetric adjacency: both directions of every edge sorted by (src, dst), the edge id riding along
+  uint64_t *d_k = nullptr, *d_k2 = nullptr;
+  uint32_t *d_id = nullptr, *d_id2 = nullptr, *d_len = nullptr;
+  LUXB_TRY(tmp.alloc(&d_k, 2 * m));
+  LUXB_TRY(tmp.alloc(&d_k2, 2 * m));
+  LUXB_TRY(tmp.alloc(&d_id, 2 * m));
+  LUXB_TRY(tmp.alloc(&d_id2, 2 * m));
+  LUXB_TRY(tmp.alloc(&d_len, nv));
+  LUXB_CUDA(cudaMemsetAsync(d_len, 0, (size_t)nv * 4, g->stream));
+  LUXB_TRY(gmalloc(g, &t.adj, 2 * m));
+  if (m) {
+    truss_emit_kernel<<<grid_for(m, 256, grid), 256, 0, g->stream>>>(t.ekey, m, d_k, d_id);
+    LUXB_CUDA(cudaGetLastError());
+    cub::DoubleBuffer<uint64_t> dk(d_k, d_k2);
+    cub::DoubleBuffer<uint32_t> di(d_id, d_id2);
+    LUXB_TRY(cub_call(tmp, g->stream, [&](void* p, size_t& b) {
+      return cub::DeviceRadixSort::SortPairs(p, b, dk, di, (long long)(2 * m), 0, bits, g->stream);
+    }));
+    truss_lists_kernel<<<grid_for(2 * m, 256, grid), 256, 0, g->stream>>>(dk.Current(), di.Current(), 2 * m, t.adj, d_len);
+    LUXB_CUDA(cudaGetLastError());
+  }
+  LUXB_TRY(gmalloc(g, &t.off, (uint64_t)nv + 1));
+  LUXB_CUDA(cudaMemsetAsync(t.off + nv, 0, 8, g->stream));
+  widen_u32_to_u64_kernel<<<grid_for(nv, 256, grid), 256, 0, g->stream>>>(d_len, t.off, nv);
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* p, size_t& b) {
+    return cub::DeviceScan::ExclusiveSum(p, b, t.off, t.off, (long long)nv + 1, g->stream);
+  }));
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  for (void* q : {(void*)d_k, (void*)d_k2, (void*)d_id, (void*)d_id2, (void*)d_len}) tmp.release(q);
+  // the run's state: support, τ (zeros until the first run), edge states, tv, alive lists, pieces, F, slots, records
+  const uint32_t n_own = t.e_hi - t.e_lo;
+  LUXB_TRY(gmalloc(g, &t.sup0, m));
+  LUXB_TRY(gmalloc(g, &t.sup, m));
+  LUXB_TRY(gmalloc(g, &t.truss, m));
+  LUXB_CUDA(cudaMemsetAsync(t.truss, 0, (size_t)m * 4, g->stream));
+  LUXB_TRY(gmalloc(g, &t.st, m));
+  LUXB_TRY(gmalloc(g, &t.tv, nv));
+  LUXB_CUDA(cudaMemsetAsync(t.tv, 0, (size_t)nv * 4, g->stream));
+  for (int i = 0; i < 2; ++i) {
+    LUXB_TRY(gmalloc(g, &t.alive[i], n_own));
+    LUXB_TRY(gmalloc(g, &t.piece[i], n_own));
+  }
+  if (g->P > 1) LUXB_TRY(gmalloc(g, &t.f, m));
+  LUXB_TRY(gmalloc(g, &t.pre, m + 1));
+  LUXB_TRY(gmalloc(g, &t.rec, 1 + LUXB_MAX_PARTS));
+  LUXB_TRY(gmalloc(g, &t.h_rec, LUXB_MAX_PARTS, MemKind::kPinned));
+  LUXB_TRY(gmalloc(g, &t.bad, 1));
+  LUXB_TRY(gmalloc(g, &t.o.next, 2));
+  LUXB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, t.scan_bytes, t.pre, t.pre, (long long)m + 1, g->stream));
+  LUXB_TRY(gmalloc(g, (char**)&t.scan_tmp, t.scan_bytes));
+  int per_sm = 0, per_sm2 = 0;
+  LUXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, truss_walk_kernel, kTrussThreads, 0));
+  LUXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm2, kcore_tally_kernel, kKcoreThreads, 0));
+  t.grid = std::max(std::min(per_sm, per_sm2), 1) * g->num_sms;
+  LUXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, truss_support_group_kernel, kTcThreads, 0));
+  t.group_grid = std::max(per_sm, 1) * g->num_sms;
+  LUXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, truss_support_big_kernel, kTcThreads, 0));
+  t.big_grid = std::max(per_sm, 1) * g->num_sms;
+  LUXB_TRY(truss_support(g));
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  return 0;
+}
+
+static int truss_handle(luxb_graph* g, const char* what) {
+  LUXB_ARG(g != nullptr, "graph is NULL");
+  if (!g->inited) { set_error("%s before luxb_init", what); return LUXB_ERR_STATE; }
+  LUXB_ARG(g->cfg.app == LUXB_TRUSS, "%s needs a LUXB_TRUSS handle (this one is app %d)", what, (int)g->cfg.app);
+  LUXB_CUDA(cudaSetDevice(g->cfg.device));
+  return 0;
+}
+
+int luxb_truss_run(luxb_graph* g, uint32_t* kmax_out) {
+  LUXB_TRY(truss_handle(g, "luxb_truss_run"));
+  LUXB_CUDA(cudaEventRecord(g->ev_begin, g->stream));
+  TrussState& t = g->tr;
+  const uint32_t n_own = t.e_hi - t.e_lo, P = (uint32_t)g->P;
+  KcoreRec* rec = t.rec;
+  LUXB_TRY(truss_support(g));
+  // every edge alive, τ unset on every rank (every rank marks the whole of F), this rank's supports from sup0
+  LUXB_CUDA(cudaMemsetAsync(t.truss, 0xFF, (size_t)t.m * 4, g->stream));
+  LUXB_CUDA(cudaMemsetAsync(t.st, kTrussAlive, t.m, g->stream));
+  const int grid = grid_for(std::max<uint32_t>(n_own, 1), 256, g->num_sms * 8);
+  kcore_reset_kernel<<<grid, 256, 0, g->stream>>>(t.truss, t.sup + t.e_lo, t.sup0 + t.e_lo, t.alive[0], n_own, t.e_lo, rec);
+  kcore_tally_kernel<<<std::min(grid, t.grid), kKcoreThreads, 0, g->stream>>>(t.alive[0], n_own, t.truss, t.sup, 0, t.alive[1], rec);
+  g->stats.kernel_launches += 2;
+  LUXB_CUDA(cudaGetLastError());
+  g->trace_active.clear();
+  g->trace_pull.clear();
+  int alive_cur = 0, piece_cur = 0;
+  uint32_t n_alive = 0, l = 0;
+  uint64_t rounds = 0;
+  std::vector<uint32_t> piece(P);
+  for (;;) {
+    // the one host synchronisation of a round: every rank's record
+    if (P > 1) LUXB_NCCL(nccl().AllGather(rec, rec + 1, sizeof(KcoreRec), ncclUint8, g->comm, g->stream));
+    LUXB_CUDA(cudaMemcpyAsync(t.h_rec, P > 1 ? rec + 1 : rec, P * sizeof(KcoreRec), cudaMemcpyDeviceToHost, g->stream));
+    LUXB_CUDA(cudaStreamSynchronize(g->stream));
+    const KcoreRec* r = t.h_rec;
+    for (uint32_t p = 0; p < P; ++p)
+      if (r[p].flag) {  // a support would have gone below zero: the schedule's invariant is broken
+        set_error("luxb_truss_run: round %llu at k = %u lowered a support of 0 on rank %u", (unsigned long long)rounds, l + 2, p);
+        return LUXB_ERR_STATE;
+      }
+    if (!r[g->cfg.rank].next) {  // the tally ran on this rank: its compacted list is current
+      alive_cur ^= 1;
+      n_alive = r[g->cfg.rank].alive;
+    }
+    uint64_t next = 0, alive = 0;
+    for (uint32_t p = 0; p < P; ++p) { next += r[p].next; alive += r[p].alive; }
+    const uint32_t* own = t.piece[piece_cur ^ 1];
+    if (next) {  // the level goes on: the pieces the walk appended
+      for (uint32_t p = 0; p < P; ++p) piece[p] = r[p].next;
+    } else {     // a new level: ℓ = the least support left, its first pieces the alive edges at that support
+      if (!alive) break;
+      uint32_t least = kKcoreUnset;
+      for (uint32_t p = 0; p < P; ++p)
+        if (r[p].alive) least = std::min(least, (uint32_t)(r[p].min_cnt >> 32));
+      l = std::max(l, least);
+      for (uint32_t p = 0; p < P; ++p) piece[p] = r[p].alive && (uint32_t)(r[p].min_cnt >> 32) == l ? (uint32_t)r[p].min_cnt : 0;
+      if (piece[g->cfg.rank]) {
+        kcore_select_kernel<<<grid_for(n_alive, 256, g->num_sms * 8), 256, 0, g->stream>>>(t.alive[alive_cur], n_alive, t.sup, 0, l,
+                                                                                          t.piece[piece_cur ^ 1], rec);
+        g->stats.kernel_launches++;
+      }
+    }
+    piece_cur ^= 1;
+    uint64_t nf = 0;
+    for (uint32_t p = 0; p < P; ++p) nf += piece[p];
+    if (!nf) {  // every rank sees the same records, so every rank stops here
+      set_error("luxb_truss_run: round %llu at k = %u has an empty F with %llu edges alive", (unsigned long long)rounds, l + 2,
+                (unsigned long long)alive);
+      return LUXB_ERR_STATE;
+    }
+    const uint32_t* f = own;
+    if (P > 1) {  // the pieces in rank order, the same empty ones skipped on every rank
+      LUXB_NCCL(nccl().GroupStart());
+      uint64_t at = 0;
+      for (uint32_t p = 0; p < P; ++p) {
+        if (piece[p])
+          LUXB_NCCL(nccl().Broadcast(p == (uint32_t)g->cfg.rank ? own : t.f + at, t.f + at, piece[p], ncclUint32, (int)p, g->comm, g->stream));
+        at += piece[p];
+      }
+      LUXB_NCCL(nccl().GroupEnd());
+      f = t.f;
+    }
+    const int fgrid = grid_for(nf + 1, 256, g->num_sms * 8);
+    truss_mark_kernel<<<fgrid, 256, 0, g->stream>>>(f, (uint32_t)nf, l + 2, t.st, t.truss, rec);
+    truss_lengths_kernel<<<fgrid, 256, 0, g->stream>>>(f, (uint32_t)nf, t.ekey, t.off, t.pre);
+    size_t scan_bytes = 0;
+    LUXB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, t.pre, t.pre, (long long)nf + 1, g->stream));
+    LUXB_ARG(scan_bytes <= t.scan_bytes, "k-truss scan needs %zu bytes of temporary storage, %zu reserved", scan_bytes, t.scan_bytes);
+    LUXB_CUDA(cub::DeviceScan::ExclusiveSum(t.scan_tmp, scan_bytes, t.pre, t.pre, (long long)nf + 1, g->stream));
+    const TrussWalkArgs wa{f, (uint32_t)nf, t.pre, t.ekey, t.off, t.adj, t.st, t.sup, t.e_lo, t.e_hi, l, t.piece[piece_cur ^ 1], rec};
+    truss_walk_kernel<<<t.grid, kTrussThreads, 0, g->stream>>>(wa);
+    truss_kill_kernel<<<fgrid, 256, 0, g->stream>>>(f, (uint32_t)nf, t.st);
+    kcore_tally_kernel<<<std::min(grid_for(std::max<uint32_t>(n_alive, 1), kKcoreThreads, g->num_sms * 8), t.grid), kKcoreThreads, 0,
+                         g->stream>>>(t.alive[alive_cur], n_alive, t.truss, t.sup, 0, t.alive[alive_cur ^ 1], rec);
+    g->stats.kernel_launches += 6;  // the scan counts as one
+    LUXB_CUDA(cudaGetLastError());
+    g->trace_active.push_back(nf);
+    g->trace_pull.push_back((int32_t)(l + 2));
+    ++rounds;
+  }
+  LUXB_TRY(truss_vertex_values(g));
+  g->stats.iterations += rounds;
+  g->stats.edges_processed += t.m;
+  LUXB_TRY(finish_timed(g));
+  if (kmax_out) *kmax_out = rounds ? l + 2 : 0;
+  return 0;
+}
+
+int luxb_truss_num_edges(const luxb_graph* g, uint64_t* m_out) {
+  LUXB_ARG(g && m_out, "NULL argument");
+  if (!g->inited) { set_error("luxb_truss_num_edges before luxb_init"); return LUXB_ERR_STATE; }
+  LUXB_ARG(g->cfg.app == LUXB_TRUSS, "luxb_truss_num_edges needs a LUXB_TRUSS handle (this one is app %d)", (int)g->cfg.app);
+  *m_out = g->tr.m;
+  return 0;
+}
+
+int luxb_truss_edges(luxb_graph* g, luxb_vid* lo, luxb_vid* hi, uint32_t* support, uint32_t* truss, uint64_t m) {
+  LUXB_TRY(truss_handle(g, "luxb_truss_edges"));
+  const TrussState& t = g->tr;
+  LUXB_ARG(m == t.m, "arrays of %llu edges, the graph has %llu", (unsigned long long)m, (unsigned long long)t.m);
+  if (m && (lo || hi)) {
+    std::vector<uint64_t> key(m);
+    LUXB_CUDA(cudaMemcpyAsync(key.data(), t.ekey, m * 8, cudaMemcpyDeviceToHost, g->stream));
+    LUXB_CUDA(cudaStreamSynchronize(g->stream));
+    for (uint64_t i = 0; i < m; ++i) {
+      if (lo) lo[i] = (uint32_t)(key[i] >> 32);
+      if (hi) hi[i] = (uint32_t)key[i];
+    }
+  }
+  if (m && support) LUXB_CUDA(cudaMemcpyAsync(support, t.sup0, m * 4, cudaMemcpyDeviceToHost, g->stream));
+  if (m && truss) LUXB_CUDA(cudaMemcpyAsync(truss, t.truss, m * 4, cudaMemcpyDeviceToHost, g->stream));
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  return 0;
+}
+
+int luxb_truss_set_truss(luxb_graph* g, const uint32_t* truss, uint64_t m) {
+  LUXB_TRY(truss_handle(g, "luxb_truss_set_truss"));
+  LUXB_ARG(truss != nullptr || m == 0, "NULL argument");
+  LUXB_ARG(m == g->tr.m, "array of %llu edges, the graph has %llu", (unsigned long long)m, (unsigned long long)g->tr.m);
+  if (m) LUXB_CUDA(cudaMemcpyAsync(g->tr.truss, truss, m * 4, cudaMemcpyHostToDevice, g->stream));
+  LUXB_TRY(truss_vertex_values(g));
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  return 0;
+}
+
+// luxb_check of a LUXB_TRUSS handle: this rank's edges that fail the truss check (truss_check_kernel)
+static int truss_check(luxb_graph* g, uint64_t* mistakes_out) {
+  const TrussState& t = g->tr;
+  LUXB_CUDA(cudaMemsetAsync(t.bad, 0, 8, g->stream));
+  if (t.e_hi > t.e_lo) {
+    truss_check_kernel<<<g->num_sms * 8, 256, 0, g->stream>>>(t.ekey, t.e_lo, t.e_hi, t.off, t.adj, t.truss, t.bad);
+    LUXB_CUDA(cudaGetLastError());
+  }
+  unsigned long long bad = 0;
+  LUXB_CUDA(cudaMemcpyAsync(&bad, t.bad, 8, cudaMemcpyDeviceToHost, g->stream));
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  *mistakes_out = bad;
+  return 0;
+}
+
 // the array luxb_get_values / luxb_set_values address: label replica, current values, betweenness scores, triangle
-// counts or core numbers
+// counts, core numbers or vertex truss numbers
 static void* values_ptr(luxb_graph* g) {
   if (app_of(g).entry == kBcRun) return g->bc.scores;
   if (g->cfg.app == LUXB_TC) return g->tc.t;
   if (g->cfg.app == LUXB_KCORE) return g->kc.core;
+  if (g->cfg.app == LUXB_TRUSS) return g->tr.tv;
   return g->d_val[g->cur];  // labels: cur stays 0
 }
 
@@ -3273,6 +3565,7 @@ int luxb_check(luxb_graph* g, uint64_t* mistakes_out) {
            "the reference has no check for pagerank / col_filter (CHECK_TASK_ID is not registered in pull_model.inl:482-521)");
   LUXB_CUDA(cudaSetDevice(g->cfg.device));
   if (g->cfg.app == LUXB_KCORE) return kcore_check(g, mistakes_out);
+  if (g->cfg.app == LUXB_TRUSS) return truss_check(g, mistakes_out);
   LUXB_CUDA(cudaMemsetAsync(g->d_counters + 1, 0, 8, g->stream));
   const uint32_t* lab = reinterpret_cast<const uint32_t*>(g->d_val[0]);
   int grid = grid_for(g->n_part, 256, g->num_sms * 8);

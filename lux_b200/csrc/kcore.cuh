@@ -33,7 +33,7 @@ struct KcoreRec {
   uint32_t next;                 // this rank's next piece (scatter appends)
   uint32_t alive;                // this rank's alive vertices after the round (tally appends)
   uint32_t sel;                  // appends of the level-start select
-  uint32_t pad;
+  uint32_t flag;                 // LUXB_TRUSS (truss.cuh): set when a decrement found support 0
   unsigned long long min_cnt;    // min deg << 32 | number of alive vertices at that deg (kKcoreNoMin when none alive)
 };
 constexpr unsigned long long kKcoreNoMin = 0xFFFFFFFF00000000ull;

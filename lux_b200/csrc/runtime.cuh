@@ -10,6 +10,7 @@
 #include "bc.cuh"
 #include "tc.cuh"
 #include "kcore.cuh"
+#include "truss.cuh"
 
 // fix-up scratch of one tiled sweep (pull.cuh): per-tile partials and carries, per-block aggregates
 struct FixupScratch {
@@ -143,6 +144,34 @@ struct KcoreState {
   int grid = 0;                    // resident CTAs of the scatter and the tally
 };
 
+// k-truss decomposition (truss.cuh): the edge table, TC's oriented lists with their edge ids, the symmetric adjacency,
+// the peel's state.  Every rank holds all of it; a rank owns the edges [e_lo, e_hi) whose lo is in its range.
+struct TrussState {
+  uint64_t m = 0;                  // undirected simple edges
+  uint32_t e_lo = 0, e_hi = 0;
+  uint64_t* ekey = nullptr;        // [m] lo << 32 | hi, ascending: the edge ids
+  TcState o;                       // oriented out-lists and this rank's bins (tc_orient_bins); o.next: work counters
+  uint32_t* oid = nullptr;         // [m] edge id of every oriented position
+  uint64_t* off = nullptr;         // [nv + 1] symmetric adjacency offsets
+  uint64_t* adj = nullptr;         // [2m] neighbour << 32 | edge id, neighbours ascending inside each list
+  uint32_t* sup0 = nullptr;        // [m] support of the input graph
+  uint32_t* sup = nullptr;         // [m] support during a run (this rank's edges current)
+  uint32_t* truss = nullptr;       // [m] τ
+  uint8_t* st = nullptr;           // [m] alive / dying / dead
+  uint32_t* tv = nullptr;          // [nv] max τ at every vertex (the handle's values)
+  uint32_t* alive[2] = {nullptr, nullptr};  // [e_hi - e_lo] alive lists of this rank's edges
+  uint32_t* piece[2] = {nullptr, nullptr};  // this rank's pieces of F
+  uint32_t* f = nullptr;           // [m] the global F (several ranks)
+  uint64_t* pre = nullptr;         // [m + 1] slot offsets of F's walks
+  luxb::KcoreRec* rec = nullptr;   // [1 + LUXB_MAX_PARTS] this rank's record, then every rank's
+  luxb::KcoreRec* h_rec = nullptr; // pinned host copy of the gathered records
+  unsigned long long* bad = nullptr;
+  void* scan_tmp = nullptr;
+  size_t scan_bytes = 0;
+  int grid = 0;                    // resident CTAs of the walk and the tally
+  int group_grid = 0, big_grid = 0;
+};
+
 // one buffer the graph keeps: device memory, pinned host memory, or pinned host memory mapped into the device's
 // address space
 enum class MemKind : uint8_t { kDevice, kPinned, kMapped };
@@ -232,6 +261,7 @@ struct luxb_graph {
   BcState bc;
   TcState tc;
   KcoreState kc;
+  TrussState tr;
 
   // communication
   luxb::ncclComm_t comm = nullptr;

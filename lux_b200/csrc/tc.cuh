@@ -17,7 +17,8 @@
 // one to the counters of w's and v's entries and to the owner's.  Counters go to t[] once per group and entry: no
 // global atomic per triangle (the hubs rank highest and are the w of most triangles).  The big kernel stages its list
 // in kTcSharedList-entry chunks and runs a warp per v of the list against each chunk.  Integers only: the result does
-// not depend on the schedule.
+// not depend on the schedule.  Both kernels are templates on where the counts go (TcVertexSink here; k-truss counts
+// edge support with the same kernels, truss.cuh).
 #pragma once
 #include <stdint.h>
 #include <cuda_runtime.h>
@@ -145,7 +146,15 @@ struct TcArgs {
   unsigned int* next;          // [2] work counters (groups, big vertices), zero at launch
 };
 
-__global__ void __launch_bounds__(kTcThreads) tc_group_kernel(const __grid_constant__ TcArgs a) {
+// Where the grouped and big kernels send what they count.  TcVertexSink: triangles per vertex into a.t (the owner's
+// share from s_own).  TrussEdgeSink (truss.cuh): support per edge, sup[eid[p]] for the oriented position p of each
+// edge of a triangle; no per-vertex share.
+struct TcVertexSink {
+  static constexpr bool kPerEdge = false;
+};
+
+template <class Sink>
+__device__ __forceinline__ void tc_group_body(const TcArgs& a, const Sink& sink) {
   typedef cub::BlockScan<uint32_t, kTcThreads> Scan;
   constexpr int kPer = kTcStage / kTcThreads;
   __shared__ uint32_t s_id[kTcStage];        // staged ids: the lists of the group's vertices, back to back
@@ -216,28 +225,42 @@ __global__ void __launch_bounds__(kTcThreads) tc_group_kernel(const __grid_const
           run_c = 0;
         }
         ++run_c;
-        if (q != run_q) {
-          if (run_o) atomicAdd(&s_own[run_q], run_o);
-          run_q = q;
-          run_o = 0;
+        if constexpr (Sink::kPerEdge) {
+          sink.add(a.off[v] + (k - s_pre[j]), 1u);  // the edge (v, w)
+        } else {
+          if (q != run_q) {
+            if (run_o) atomicAdd(&s_own[run_q], run_o);
+            run_q = q;
+            run_o = 0;
+          }
+          ++run_o;
         }
-        ++run_o;
       }
     }
     if (run_c) atomicAdd(&s_cnt[run_j], run_c);
-    if (run_o) atomicAdd(&s_own[run_q], run_o);
+    if constexpr (!Sink::kPerEdge) {
+      if (run_o) atomicAdd(&s_own[run_q], run_o);
+    }
     __syncthreads();
-    for (uint32_t i = tid; i < S; i += kTcThreads)
-      if (s_cnt[i]) atomicAdd(a.t + s_id[i], (unsigned long long)s_cnt[i]);
-    for (uint32_t q = tid; q < nq; q += kTcThreads)
-      if (s_own[q]) atomicAdd(a.t + a.staged[k0 + q], (unsigned long long)s_own[q]);
+    if constexpr (Sink::kPerEdge) {  // entry i is the edge (owner, s_id[i])
+      for (uint32_t i = tid; i < S; i += kTcThreads)
+        if (s_cnt[i]) sink.add(a.off[a.staged[k0 + s_q[i]]] + (i - s_sp[s_q[i]]), s_cnt[i]);
+    } else {
+      for (uint32_t i = tid; i < S; i += kTcThreads)
+        if (s_cnt[i]) atomicAdd(a.t + s_id[i], (unsigned long long)s_cnt[i]);
+      for (uint32_t q = tid; q < nq; q += kTcThreads)
+        if (s_own[q]) atomicAdd(a.t + a.staged[k0 + q], (unsigned long long)s_own[q]);
+    }
     __syncthreads();  // shared memory is restaged by the next group
   }
 }
 
+__global__ void __launch_bounds__(kTcThreads) tc_group_kernel(const __grid_constant__ TcArgs a) { tc_group_body(a, TcVertexSink{}); }
+
 // one CTA per big vertex u: N+(u) staged kTcSharedList entries at a time; a warp per v in N+(u) probes N+(v) against
 // the chunk.  c(u, v) goes to t[v] once per chunk and v, the chunk's counters to t[w], the sum of c to t[u]
-__global__ void __launch_bounds__(kTcThreads) tc_big_kernel(const __grid_constant__ TcArgs a) {
+template <class Sink>
+__device__ __forceinline__ void tc_big_body(const TcArgs& a, const Sink& sink) {
   __shared__ uint32_t s_id[kTcSharedList];
   __shared__ uint32_t s_cnt[kTcSharedList];
   __shared__ unsigned long long s_own;
@@ -277,25 +300,39 @@ __global__ void __launch_bounds__(kTcThreads) tc_big_kernel(const __grid_constan
           if (b < cn && s_id[b] == w) {
             atomicAdd(&s_cnt[b], 1u);
             ++c;
+            if constexpr (Sink::kPerEdge) sink.add(vb + p, 1u);  // the edge (v, w)
           }
         }
 #pragma unroll
         for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xFFFFFFFFu, c, o);
         if (lane == 0 && c) {
-          atomicAdd(a.t + v, (unsigned long long)c);
-          own += c;
+          if constexpr (Sink::kPerEdge) {
+            sink.add(ub + j, c);  // the edge (u, v)
+          } else {
+            atomicAdd(a.t + v, (unsigned long long)c);
+            own += c;
+          }
         }
       }
       __syncthreads();
-      for (uint32_t i = tid; i < cn; i += kTcThreads)
-        if (s_cnt[i]) atomicAdd(a.t + s_id[i], (unsigned long long)s_cnt[i]);
+      for (uint32_t i = tid; i < cn; i += kTcThreads) {
+        if constexpr (Sink::kPerEdge) {
+          if (s_cnt[i]) sink.add(ub + c0 + i, s_cnt[i]);  // the edge (u, w)
+        } else {
+          if (s_cnt[i]) atomicAdd(a.t + s_id[i], (unsigned long long)s_cnt[i]);
+        }
+      }
       __syncthreads();  // the next chunk overwrites s_id / s_cnt
     }
-    if (own) atomicAdd(&s_own, own);
-    __syncthreads();
-    if (tid == 0 && s_own) atomicAdd(a.t + u, s_own);
+    if constexpr (!Sink::kPerEdge) {
+      if (own) atomicAdd(&s_own, own);
+      __syncthreads();
+      if (tid == 0 && s_own) atomicAdd(a.t + u, s_own);
+    }
     __syncthreads();  // s_own / s_b are reset for the next vertex
   }
 }
+
+__global__ void __launch_bounds__(kTcThreads) tc_big_kernel(const __grid_constant__ TcArgs a) { tc_big_body(a, TcVertexSink{}); }
 
 }  // namespace luxb

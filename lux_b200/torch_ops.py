@@ -1,4 +1,4 @@
-"""PyTorch front-end of the C ABI (SURVEY §8 f4): the four Lux apps, weighted SSSP, betweenness centrality, triangle counting and k-core decomposition as `torch.ops.luxb.*` custom ops taking the CSC as
+"""PyTorch front-end of the C ABI (SURVEY §8 f4): the four Lux apps, weighted SSSP, betweenness centrality, triangle counting, k-core decomposition and k-truss decomposition as `torch.ops.luxb.*` custom ops taking the CSC as
 torch tensors and returning torch tensors.  Plumbing only — every op opens a libluxb handle through the ctypes binding
 (lux_b200/binding.py), runs the app on the CUDA device of the current torch context and copies the result back; no torch
 kernel takes part in the computation, and there is no CPU fallback (the ops raise without a GPU).
@@ -13,6 +13,7 @@ kernel takes part in the computation, and there is no CPU fallback (the ops rais
     bc     = torch.ops.luxb.betweenness_weighted(row_end, src, weight, sources)  # f64 [nv]  (weighted paths, weights >= 1)
     t      = torch.ops.luxb.triangles(row_end, src)             # i64 [nv]  (triangles at each vertex, undirected simple graph)
     core   = torch.ops.luxb.core_number(row_end, src)           # i64 [nv]  (core number of each vertex, undirected simple graph)
+    edges, truss = torch.ops.luxb.k_truss(row_end, src)         # i64 [m, 2] (lo, hi ascending), i64 [m] truss numbers
 row_end: int64 [nv] END offsets (the .lux convention); src: int64/int32 [ne]; weight: int32 [ne]; sources: int64/int32 [k] vertex ids."""
 import numpy as np
 import torch
@@ -38,6 +39,7 @@ _lib.define("betweenness(Tensor row_end, Tensor src, Tensor sources) -> Tensor")
 _lib.define("betweenness_weighted(Tensor row_end, Tensor src, Tensor weight, Tensor sources) -> Tensor")
 _lib.define("triangles(Tensor row_end, Tensor src) -> Tensor")
 _lib.define("core_number(Tensor row_end, Tensor src) -> Tensor")
+_lib.define("k_truss(Tensor row_end, Tensor src) -> (Tensor, Tensor)")
 
 
 def _pagerank(row_end, src, num_iter):
@@ -88,7 +90,13 @@ def _core_number(row_end, src):
     return torch.from_numpy(out["core"].astype(np.int64)).to(row_end.device)
 
 
+def _k_truss(row_end, src):
+    out = _apps.truss(_np(row_end, np.uint64), _np(src, np.uint32), device=_device_index(row_end))
+    edges = np.stack([out["lo"], out["hi"]], axis=1).astype(np.int64).reshape(-1, 2)
+    return torch.from_numpy(edges).to(row_end.device), torch.from_numpy(out["truss"].astype(np.int64)).to(row_end.device)
+
+
 for _name, _fn in (("pagerank", _pagerank), ("components", _components), ("sssp", _sssp), ("colfilter", _colfilter),
                    ("sssp_weighted", _sssp_weighted), ("betweenness", _betweenness), ("betweenness_weighted", _betweenness_weighted),
-                   ("triangles", _triangles), ("core_number", _core_number)):
+                   ("triangles", _triangles), ("core_number", _core_number), ("k_truss", _k_truss)):
     _lib.impl(_name, _fn, "CompositeExplicitAutograd")
