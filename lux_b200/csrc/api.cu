@@ -7,6 +7,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <algorithm>
+#include <type_traits>
 #include <new>
 
 #include "build.cuh"
@@ -1366,7 +1367,7 @@ static void fill_fixup_args(PullArgs<Prog>& a, const FixupScratch& f) {
 
 // f is the sweep's own scratch (the fused fix-up keeps its launch epoch there)
 template <class Prog>
-static int launch_fixup(luxb_graph* g, const PullArgs<Prog>& a, FixupScratch& f) {
+static int launch_fixup(luxb_graph* g, const PullArgs<Prog>& a, FixupScratch& f, const uint2* piece_slot = nullptr) {
   if (a.n_tiles <= 1) return 0;
   if (g->fused_fixup) {
     if (!f.d_chain) {
@@ -1384,14 +1385,14 @@ static int launch_fixup(luxb_graph* g, const PullArgs<Prog>& a, FixupScratch& f)
       LUXB_CUDA(cudaMemsetAsync(f.d_chain, 0, (4ull * f.n_fix_blocks + 4) * 8, g->stream));
       f.chain_epoch = ch.epoch = 1;
     }
-    pull_fixup_fused_kernel<Prog><<<f.n_fix_blocks, kFixBlock, 0, g->stream>>>(a, ch);
+    pull_fixup_fused_kernel<Prog><<<f.n_fix_blocks, kFixBlock, 0, g->stream>>>(a, ch, piece_slot);
     LUXB_CUDA(cudaGetLastError());
     g->stats.kernel_launches++;
     return 0;
   }
   pull_fixup_scan_kernel<Prog><<<f.n_fix_blocks, kFixBlock, 0, g->stream>>>(a);
   pull_fixup_blocks_kernel<Prog><<<1, 1024, 0, g->stream>>>(a, f.n_fix_blocks);
-  pull_fixup_apply_kernel<Prog><<<f.n_fix_blocks, kFixBlock, 0, g->stream>>>(a);
+  pull_fixup_apply_kernel<Prog><<<f.n_fix_blocks, kFixBlock, 0, g->stream>>>(a, piece_slot);
   LUXB_CUDA(cudaGetLastError());
   g->stats.kernel_launches += 3;
   return 0;
@@ -1499,10 +1500,12 @@ extern "C++" {
 // wbase / hshift are filled here).  Every block is padded with 1 .. stage_edges head-flagged dummy words to a whole
 // number of stages.  On return L holds words, close list, tile_v (heads before each piece), fix-up scratch and, if
 // want_empty, the list of vertices without edges.  super_end (optional) receives the first stage after each block.
+// slots: a group stream (panel.cuh) — no close list; its non-empty "vertices" are the compact slots slot_base,
+// slot_base + 1, ... in order, L.d_piece_slot says which of them each piece closes and L.n_slots counts them.
 template <class Word, class In>
 static int build_seg_stream(luxb_graph* g, PullLayout& L, const uint64_t* d_row_end, uint32_t n_vtx, const In* d_ids, uint64_t e_cnt,
-                            StreamBlocks& blk, uint32_t stage_edges, uint32_t piece, uint32_t vtx_offset, bool want_empty,
-                            const uint32_t* hub_bits, uint32_t* super_end) {
+                            StreamBlocks& blk, uint32_t stage_edges, uint32_t piece, bool want_empty, const uint32_t* hub_bits,
+                            uint32_t* super_end, bool slots = false, uint32_t slot_base = 0) {
   const int grid = g->num_sms * 8;
   DevTmp tmp;
   L = PullLayout();
@@ -1536,7 +1539,8 @@ static int build_seg_stream(luxb_graph* g, PullLayout& L, const uint64_t* d_row_
   uint32_t n_seg = 0;
   LUXB_CUDA(cudaMemcpyAsync(&n_seg, d_rank + n_vtx, 4, cudaMemcpyDeviceToHost, g->stream));
   LUXB_CUDA(cudaStreamSynchronize(g->stream));
-  // 2. words: ids, then pads, then head flags; close list (entry j + 1 = owner of head j, dummies for the pads)
+  // 2. words: ids, then pads, then head flags; close list (entry j + 1 = owner of head j, dummies for the pads) unless
+  // the heads close compact slots
   Word* d_words = nullptr;
   LUXB_TRY(gmalloc(g, &d_words, words + 64));
   L.d_src = d_words;
@@ -1548,9 +1552,11 @@ static int build_seg_stream(luxb_graph* g, PullLayout& L, const uint64_t* d_row_
   LUXB_CUDA(cudaGetLastError());
   const uint64_t n_heads = (uint64_t)n_seg + pads_total;
   LUXB_ARG(n_heads < 0xFFFFFFF0ull, "too many segments");
-  LUXB_TRY(gmalloc(g, &L.d_close, n_heads + 2));
-  LUXB_CUDA(cudaMemsetAsync(L.d_close, 0xFF, (n_heads + 2) * 4, g->stream));
-  stream_heads_kernel<Word><<<grid, 256, 0, g->stream>>>(d_row_end, n_vtx, d_flag, d_rank, blk, d_words, L.d_close, vtx_offset);
+  if (!slots) {
+    LUXB_TRY(gmalloc(g, &L.d_close, n_heads + 2));
+    LUXB_CUDA(cudaMemsetAsync(L.d_close, 0xFF, (n_heads + 2) * 4, g->stream));
+  }
+  stream_heads_kernel<Word><<<grid, 256, 0, g->stream>>>(d_row_end, n_vtx, d_flag, d_rank, blk, d_words, L.d_close);
   LUXB_CUDA(cudaGetLastError());
   // 3. heads before each piece
   uint32_t* d_cnt = nullptr;
@@ -1564,6 +1570,13 @@ static int build_seg_stream(luxb_graph* g, PullLayout& L, const uint64_t* d_row_
   }));
   uint32_t heads_counted = 0;
   LUXB_CUDA(cudaMemcpyAsync(&heads_counted, L.d_tile_v + L.n_tiles, 4, cudaMemcpyDeviceToHost, g->stream));
+  if (slots) {
+    LUXB_ARG((uint64_t)slot_base + n_seg < 0x7FFFFFF0ull, "too many slots");
+    LUXB_TRY(gmalloc(g, &L.d_piece_slot, (uint64_t)L.n_tiles + 1));
+    piece_slot_kernel<<<grid_for(L.n_tiles, 256, grid), 256, 0, g->stream>>>(L.d_tile_v, L.n_tiles, piece, d_rank, blk, slot_base, L.d_piece_slot);
+    LUXB_CUDA(cudaGetLastError());
+    L.n_slots = n_seg;
+  }
   // 4. vertices without edges (hubs among them apart)
   unsigned int* d_cur2 = nullptr;
   if (want_empty) {
@@ -1599,17 +1612,19 @@ static int build_main_stream(luxb_graph* g, const uint64_t* d_row_end, const uin
   blk.vfirst[1] = g->n_part;
   blk.ebase[1] = e_cnt;
   return build_seg_stream<uint32_t, uint32_t>(g, g->sb_main, d_row_end, g->n_part, d_ids, e_cnt, blk, (uint32_t)shp.stage_edges,
-                                              (uint32_t)shp.piece, 0, true, hub_bits, nullptr);
+                                              (uint32_t)shp.piece, true, hub_bits, nullptr);
 }
 
 extern "C++" {
 // The flagged stream of the split's groups [g0, g1) (panel.cuh): their e_cnt sorted edges (d_key / d_pay) -> ids
-// (group_fill_kernel), the CSC over their slots vbase[g0] .. vbase[g1] - 1, and the stream, whose close list holds the
-// slot numbers.  With super_end every group is padded to whole stages (the panel: a stage never straddles two source
+// (group_fill_kernel), the CSC over their dense (group, hub) pairs vbase[g0] .. vbase[g1] - 1, their words of the slot
+// bitmap d_bits, and the stream, whose heads close the compact slots slot_base, slot_base + 1, ... (the non-empty pairs
+// in order).  With super_end every group is padded to whole stages (the panel: a stage never straddles two source
 // blocks) and super_end receives the first stage after each; without, the groups form one block.
 template <class Word>
 static int build_group_stream(luxb_graph* g, PullLayout& L, const uint16_t* d_key, const uint64_t* d_pay, uint64_t e_cnt, uint32_t g0,
-                              uint32_t g1, const unsigned long long* hist, uint32_t bs, const SegShapeInfo& shp, uint32_t* super_end) {
+                              uint32_t g1, const unsigned long long* hist, uint32_t bs, const SegShapeInfo& shp, uint32_t* super_end,
+                              uint32_t* d_bits, uint32_t slot_base) {
   const int grid = g->num_sms * 8;
   const uint32_t* vbase = g->sb_groups.vbase;
   const uint32_t v0 = vbase[g0], n_vtx = vbase[g1] - v0;
@@ -1627,6 +1642,8 @@ static int build_group_stream(luxb_graph* g, PullLayout& L, const uint16_t* d_ke
   LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
     return cub::DeviceScan::InclusiveSum(t, b, d_vrow, d_vrow, (int)n_vtx, g->stream);
   }));
+  slot_bits_kernel<<<grid, 256, 0, g->stream>>>(d_vcount, g->sb_groups, g0, g1, v0, d_bits);
+  LUXB_CUDA(cudaGetLastError());
   tmp.release(d_vcount);
   StreamBlocks blk{};
   blk.n_blocks = super_end ? g1 - g0 : 1;
@@ -1634,8 +1651,8 @@ static int build_group_stream(luxb_graph* g, PullLayout& L, const uint16_t* d_ke
     blk.vfirst[b + 1] = super_end ? vbase[g0 + b + 1] - v0 : n_vtx;
     blk.ebase[b + 1] = super_end ? blk.ebase[b] + hist[g0 + b] : e_cnt;
   }
-  return build_seg_stream<Word, Word>(g, L, d_vrow, n_vtx, d_ids, e_cnt, blk, (uint32_t)shp.stage_edges, (uint32_t)shp.piece, v0, false,
-                                      nullptr, super_end);
+  return build_seg_stream<Word, Word>(g, L, d_vrow, n_vtx, d_ids, e_cnt, blk, (uint32_t)shp.stage_edges, (uint32_t)shp.piece, false,
+                                      nullptr, super_end, true, slot_base);
 }
 }  // extern "C++"
 
@@ -1801,22 +1818,45 @@ static int build_panel_layout(luxb_graph* g) {
   }
   if (e_cov == 0 || (st.sb < 0 && e_cov < g->e_part / 5)) return 0;
 
-  // 4. the group table: block b serves N_b hubs, a cold segment all Nh; slot vbase[g] + h
+  // 4. the group table: block b serves N_b hubs, a cold segment all Nh; dense pair vbase[g] + h, bitmap words from
+  // wbase[g]
   const uint32_t NG = NB + S;
   LUXB_ARG(NG < kSplitKeyMain, "panel: too many source groups");
-  uint64_t n_slots = 0;
+  uint64_t n_pairs = 0, n_words = 0;
   g->sb_groups = SplitGroups{};
   for (uint32_t k = 0; k < NG; ++k) {
-    n_slots += k < NB ? n_pref[k] : Nh;
-    LUXB_ARG(n_slots < 0x7FFFFFF0ull, "panel: too many (group, hub) slots");
-    g->sb_groups.vbase[k + 1] = (uint32_t)n_slots;
+    const uint32_t n_k = k < NB ? n_pref[k] : Nh;
+    n_pairs += n_k;
+    n_words += (n_k + 31) / 32;
+    LUXB_ARG(n_pairs < 0x7FFFFFF0ull, "panel: too many (group, hub) pairs");
+    g->sb_groups.vbase[k + 1] = (uint32_t)n_pairs;
+    g->sb_groups.wbase[k + 1] = (uint32_t)n_words;
   }
+  uint32_t *d_slot_bits = nullptr, *d_slot_pre = nullptr;
+  LUXB_TRY(tmp.alloc(&d_slot_bits, n_words + 1));
+  LUXB_TRY(tmp.alloc(&d_slot_pre, n_words + 1));
   // 5. the panel (per-block stage padding) and the cold-hub stream (one block: its kernel claims stages in order, so the
-  // SMs move through the segments together)
-  LUXB_TRY(build_group_stream<uint16_t>(g, g->sb_panel, d_key2, d_pay2, e_cov, 0, NB, hist, bs, shp, g->sb_super_end));
+  // SMs move through the segments together); the cold-hub slots follow the panel's
+  LUXB_TRY(build_group_stream<uint16_t>(g, g->sb_panel, d_key2, d_pay2, e_cov, 0, NB, hist, bs, shp, g->sb_super_end, d_slot_bits, 0));
   if (S)
     LUXB_TRY(build_group_stream<uint32_t>(g, g->sb_cold, d_key2 + e_cov, d_pay2 + e_cov, e_cold, NB, NG, hist, 0,
-                                          kSegMainInfo[st.cs_shape], nullptr));
+                                          kSegMainInfo[st.cs_shape], nullptr, d_slot_bits, g->sb_panel.n_slots));
+  const uint64_t n_slots = (uint64_t)g->sb_panel.n_slots + (S ? g->sb_cold.n_slots : 0);
+  // the combine's prefix: slots before each bitmap word, = the streams' numbering
+  popc_kernel<<<grid, 256, 0, g->stream>>>(d_slot_bits, n_words, d_slot_pre);
+  LUXB_CUDA(cudaMemsetAsync(d_slot_pre + n_words, 0, 4, g->stream));
+  LUXB_CUDA(cudaGetLastError());
+  LUXB_TRY(cub_call(tmp, g->stream, [&](void* t, size_t& b) {
+    return cub::DeviceScan::ExclusiveSum(t, b, d_slot_pre, d_slot_pre, (int)n_words + 1, g->stream);
+  }));
+  uint32_t kind_slots[4] = {0, 0, 0, 0};  // slots before tier 0, the tiers, the cold segments, the end
+  const uint32_t kind_word[4] = {0, g->sb_groups.wbase[NB0], g->sb_groups.wbase[NB], (uint32_t)n_words};
+  for (int i = 0; i < 4; ++i) LUXB_CUDA(cudaMemcpyAsync(&kind_slots[i], d_slot_pre + kind_word[i], 4, cudaMemcpyDeviceToHost, g->stream));
+  LUXB_CUDA(cudaStreamSynchronize(g->stream));
+  if ((uint64_t)kind_slots[3] != n_slots) {
+    set_error("panel split: %u slots in the bitmap, %llu in the streams", kind_slots[3], (unsigned long long)n_slots);
+    return LUXB_ERR_STATE;
+  }
 
   // 6. main stream: what is left, in the original (dst, src) order
   uint32_t* d_main_src = nullptr;
@@ -1839,13 +1879,12 @@ static int build_panel_layout(luxb_graph* g) {
   tmp.release(d_main_row);
   tmp.release(d_main_src);
 
-  // 7. raw sums of every (group, hub) slot; slots without edges keep the program's identity forever (0 bits for sums
-  // and max labels, all ones for min distances; the cold-hub stream is PageRank only)
+  // 7. raw sums of every slot: each sweep of the group streams writes all of them (pairs without edges have none)
   LUXB_TRY(gmalloc(g, &g->d_sb_partial, (uint64_t)n_slots + 1));
-  LUXB_CUDA(cudaMemsetAsync(g->d_sb_partial, g->cfg.app == LUXB_SSSP || g->cfg.app == LUXB_BC ? 0xFF : 0, ((size_t)n_slots + 1) * 4, g->stream));
-  LUXB_CUDA(cudaStreamSynchronize(g->stream));
   g->d_hub_vtx = d_hub_vtx; tmp.keep(g, d_hub_vtx);
   g->d_hub_bits = d_hub_bits; tmp.keep(g, d_hub_bits);
+  g->d_slot_bits = d_slot_bits; tmp.keep(g, d_slot_bits);
+  g->d_slot_pre = d_slot_pre; tmp.keep(g, d_slot_pre);
   g->sb_n_hub = Nh;
   g->sb_n_blocks = NB;
   g->sb_n_groups = NG;
@@ -1861,11 +1900,15 @@ static int build_panel_layout(luxb_graph* g) {
   g->stats.tier_blocks = NB - NB0;
   g->stats.tier_slots = NV - (uint64_t)NB0 * Nh;
   g->stats.tier_edges = e_cov - e_cov0;
-  if (g->cfg.verbose)
+  if (g->cfg.verbose) {
     printf("[luxb rank %d] source-blocked sweep: %u hub destinations (in-degree >= %u) x %u blocks of %u hot sources, + %u tier blocks "
            "(%llu slots, %llu edges); panel %llu edges (%.1f %%), cold-hub %llu edges (%u segments of %u values), main %llu edges\n",
            g->cfg.rank, Nh, st.sb_min_indeg, NB0, bs, NB - NB0, (unsigned long long)(NV - (uint64_t)NB0 * Nh), (unsigned long long)(e_cov - e_cov0),
            (unsigned long long)e_cov, 100.0 * e_cov / g->e_part, (unsigned long long)e_cold, S, cs.seg, (unsigned long long)e_main);
+    printf("[luxb rank %d] (group, hub) pairs with edges / all: tier 0 %u / %llu, tiers %u / %llu, cold segments %u / %llu\n", g->cfg.rank,
+           kind_slots[1], (unsigned long long)NB0 * Nh, kind_slots[2] - kind_slots[1], (unsigned long long)(NV - (uint64_t)NB0 * Nh),
+           kind_slots[3] - kind_slots[2], (unsigned long long)Nh * S);
+  }
   return 0;
 }
 
@@ -1901,20 +1944,22 @@ static int launch_seg_shape(luxb_graph* g, const SegArgs<Prog>& a, int ctas_per_
 
 // one flagged stream L (seg.cuh): the seg kernel in shape `shape` of the panel (kPanel) or the main family, then its
 // fix-up.  The caller has set a's stream-specific fields; L's own arrays are filled here.  counter_slot: the stream's
-// tile counter in d_counters; tag: the phase-timer slot of the kernel.
-template <bool kPanel, class Prog>
+// tile counter in d_counters; tag: the phase-timer slot of the kernel.  kSlots: a main shape over a group stream
+// (the cold-hub stream; the panel always is one).
+template <bool kPanel, class Prog, bool kSlots = kPanel>
 static int launch_seg_stream(luxb_graph* g, PullLayout& L, SegArgs<Prog>& a, int shape, int ctas_per_sm, int counter_slot, int tag,
                              const char* name) {
   a.p.tile_v = L.d_tile_v;
   a.p.n_tiles = L.n_tiles;
   fill_fixup_args(a.p, L.fix);
   a.p.close_vtx = L.d_close;
+  a.piece_slot = L.d_piece_slot;
   a.words = L.d_src;
   a.n_stages = L.n_stages;
   a.tile_counter = reinterpret_cast<uint32_t*>(g->d_counters + counter_slot);
   LUXB_CUDA(cudaMemsetAsync(a.tile_counter, 0, 4, g->stream));
 #define LUXB_CASE_MSHAPE(id, warps, stages, rounds) \
-  case id: LUXB_TRY((launch_seg_shape<Prog, SegMain##id>(g, a, ctas_per_sm))); break;
+  case id: LUXB_TRY((launch_seg_shape<Prog, std::conditional_t<kSlots, SlotShape<SegMain##id>, SegMain##id>>(g, a, ctas_per_sm))); break;
 #define LUXB_CASE_PSHAPE(id, warps, stages, rounds, tab, v) \
   case id: LUXB_TRY((launch_seg_shape<Prog, SegPanel##id>(g, a, ctas_per_sm))); break;
   if constexpr (kPanel) {
@@ -1930,7 +1975,7 @@ static int launch_seg_stream(luxb_graph* g, PullLayout& L, SegArgs<Prog>& a, int
   }
   g->stats.kernel_launches++;
   pt_mark(g, tag);
-  return launch_fixup(g, a.p, L.fix);
+  return launch_fixup(g, a.p, L.fix, L.d_piece_slot);
 }
 }  // extern "C++"
 
@@ -1990,17 +2035,23 @@ static int sweep_seg(luxb_graph* g, const typename Prog::Vertex* x_nat, const ty
   }
   if (g->cs_on) {
     // cold-hub stream: raw partial per (cold segment, hub) slot; its gathers all index the compact cold values, which it
-    // loads with evict_normal (l2_hints = 0): the current segment is meant to stay in L2 while the SMs sweep it
-    SegArgs<Prog> ca{};
-    ca.p.x_old = x_cold;
-    ca.p.x_hot = reinterpret_cast<const typename Prog::Vertex*>(g->d_hot);
-    ca.p.hot_n = g->hot_n;
-    ca.p.out = reinterpret_cast<typename Prog::Vertex*>(g->d_sb_partial);
-    ca.p.raw_out = 1;
-    ca.p.l2_hints = 0;
-    ca.p.prm = prm;
-    LUXB_TRY((launch_seg_stream<false, Prog>(g, g->sb_cold, ca, g->sweep.cs_shape, g->pull_ctas, 4, 9, "cold-hub")));
-    pt_mark(g, 1);
+    // loads with evict_normal (l2_hints = 0): the current segment is meant to stay in L2 while the SMs sweep it.  Only
+    // PageRank builds it (the compact cold copy is PageRank's), so only PageRank instantiates its kernels.
+    if constexpr (std::is_same<Prog, PageRankProgram>::value) {
+      SegArgs<Prog> ca{};
+      ca.p.x_old = x_cold;
+      ca.p.x_hot = reinterpret_cast<const typename Prog::Vertex*>(g->d_hot);
+      ca.p.hot_n = g->hot_n;
+      ca.p.out = reinterpret_cast<typename Prog::Vertex*>(g->d_sb_partial);
+      ca.p.raw_out = 1;
+      ca.p.l2_hints = 0;
+      ca.p.prm = prm;
+      LUXB_TRY((launch_seg_stream<false, Prog, true>(g, g->sb_cold, ca, g->sweep.cs_shape, g->pull_ctas, 4, 9, "cold-hub")));
+      pt_mark(g, 1);
+    } else {
+      set_error("the cold-hub stream is built for PageRank only");
+      return LUXB_ERR_STATE;
+    }
   }
   LUXB_TRY((launch_seg_main<Prog>(g, g->sb_main, x_nat, x_cold, out_local, out_buffer, prm, g->sb_on ? g->d_hub_bits : nullptr)));
   LUXB_TRY(kt_end(g));
@@ -2012,6 +2063,8 @@ static int sweep_seg(luxb_graph* g, const typename Prog::Vertex* x_nat, const ty
     ca.n_groups = g->sb_n_groups;
     ca.row_left = g->row_left;
     ca.sg = g->sb_groups;
+    ca.slot_bits = g->d_slot_bits;
+    ca.slot_pre = g->d_slot_pre;
     ca.partial = reinterpret_cast<const Acc*>(g->d_sb_partial);
     ca.x_nat = x_nat;
     ca.out = out_local;

@@ -16,8 +16,12 @@
 //     its in-edges stored as 15-BIT offsets into block b plus a head flag — 2 B of edge stream instead of 4 B.  Blocks
 //     are padded to whole stages, so a stage never straddles two blocks.
 //   * source GROUPS: group g < NB is panel block g, group NB + s is cold segment s (ColdSplit).  Group g serves the hub
-//     prefix [0, N_g) (N_g = Nh for a segment) and owns the "virtual vertices" (slots) vbase[g] + h, h < N_g
-//     (SplitGroups); the group number is the edge's sort key.
+//     prefix [0, N_g) (N_g = Nh for a segment); the group number is the edge's sort key.  A (group, hub) pair with at
+//     least one edge is a SLOT.  Slots are numbered compactly and implicitly: groups ascending, hubs ascending inside a
+//     group — the order in which the group streams close them — so a stream needs no close list (seg.cuh: slot0 +
+//     head index per piece), and pairs without edges cost nothing.  The slot bitmap (one bit per (g, h < N_g), 32-hub
+//     words, ceil(N_g / 32) words from SplitGroups::wbase[g]) and its per-word prefix of set bits give the combine the
+//     slot of (g, h): pre[w] + popc(bits[w] & lanes below h).
 // The panel stream is swept by seg_tile_kernel<kPanel> (seg.cuh): its producer warp keeps block b's values resident in
 // shared memory (one TMA bulk load of BS * 4 B from the hot copies per block change) and its gathers are ld.shared.  It
 // and the cold-hub stream write RAW partial sums into one array of slots.  The remaining edges stay in the "main"
@@ -38,7 +42,9 @@ constexpr uint16_t kSplitKeyMain = 511;
 constexpr int kSplitKeyBits = 9;
 
 struct SplitGroups {
-  uint32_t vbase[kSplitKeyMain + 1];  // first slot of group g; [n_groups] = all slots
+  uint32_t vbase[kSplitKeyMain + 1];  // Σ_{g' < g} N_g': N_g = vbase[g + 1] - vbase[g]; the dense (g, h) index vbase[g] + h
+                                      // numbers the per-pair edge counts during construction
+  uint32_t wbase[kSplitKeyMain + 1];  // first word of group g in the slot bitmap; [n_groups] = all words
 };
 
 // ---- one-time construction of the panel / main split --------------------------------------------------------------
@@ -148,8 +154,8 @@ __global__ void key_hist_kernel(const uint16_t* __restrict__ key, uint64_t n, un
     if (s_h[i]) atomicAdd(hist + i, (unsigned long long)s_h[i]);
 }
 
-// sorted (by group, stable) edges of groups starting at slot v0 -> their ids (gather id - group * bs: 16-bit block
-// offsets for the panel, bs = 0 keeps the gather ids) + the in-degree of every slot, counted from v0
+// sorted (by group, stable) edges of groups starting at dense pair v0 -> their ids (gather id - group * bs: 16-bit block
+// offsets for the panel, bs = 0 keeps the gather ids) + the edge count of every (group, hub) pair, counted from v0
 template <class Word>
 __global__ void group_fill_kernel(const uint16_t* __restrict__ key_sorted, const uint64_t* __restrict__ payload_sorted, uint64_t e_cnt,
                                   const uint32_t* __restrict__ src_gather, uint32_t bs, const __grid_constant__ SplitGroups sg,
@@ -180,6 +186,29 @@ __global__ void main_indeg_kernel(const uint64_t* __restrict__ row_end_rel, uint
   }
 }
 
+// slot bitmap of groups [g0, g1) from the edge counts of their dense (group, hub) pairs (vcount, counted from pair v0):
+// one warp per 32-hub word; bits past N_g stay clear
+__global__ void slot_bits_kernel(const uint32_t* __restrict__ vcount, const __grid_constant__ SplitGroups sg, uint32_t g0, uint32_t g1,
+                                 uint32_t v0, uint32_t* __restrict__ bits) {
+  const unsigned lane = threadIdx.x & 31;
+  const uint64_t warps_total = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+  for (uint64_t w = sg.wbase[g0] + (((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5); w < sg.wbase[g1]; w += warps_total) {
+    uint32_t lo = g0, hi = g1;  // the group of word w: sg.wbase[lo] <= w < sg.wbase[hi]
+    while (hi - lo > 1) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (sg.wbase[mid] <= w) lo = mid; else hi = mid;
+    }
+    const uint32_t h = (uint32_t)(w - sg.wbase[lo]) * 32u + lane;
+    const bool f = h < sg.vbase[lo + 1] - sg.vbase[lo] && vcount[sg.vbase[lo] - v0 + h] != 0;
+    const unsigned m = __ballot_sync(0xffffffffu, f);
+    if (lane == 0) bits[w] = m;
+  }
+}
+
+__global__ void popc_kernel(const uint32_t* __restrict__ bits, uint64_t n, uint32_t* __restrict__ out) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) out[i] = __popc(bits[i]);
+}
+
 // ---- per-iteration: hubs = main raw sum + panel partials (blocks b with h < N_b) + cold-segment partials, fp64, fixed
 // order; then update() ---
 template <class Prog>
@@ -187,12 +216,16 @@ struct CombineArgs {
   const uint32_t* hub_vtx;   // [n_hub] local vertex ids
   uint32_t n_hub, n_blocks, n_groups, row_left;
   SplitGroups sg;
-  const typename Prog::Acc* partial;  // raw reductions, slot vbase[g] + h
+  const uint32_t* slot_bits;  // [sg.wbase[n_groups]] bit h % 32 of word wbase[g] + h / 32: (g, h) has a slot
+  const uint32_t* slot_pre;   // [sg.wbase[n_groups]] slots before the word (set bits of all earlier words)
+  const typename Prog::Acc* partial;  // raw reductions, one per slot
   const typename Prog::Vertex* x_nat; // natural-order values of the previous iteration (update()'s old value)
   typename Prog::Vertex* out;  // [n_part] local; holds the main kernel's RAW sum for hub vertices on entry
   typename Prog::Params prm;
 };
 
+// A pair (g, h) without a slot has no edges: its partial would be the program's identity, which combines exactly (+0.0
+// for PageRank's non-negative sums, the identity of max / min for labels), so skipping it changes no bit.
 template <class Prog>
 __global__ void combine_hub_kernel(const __grid_constant__ CombineArgs<Prog> a) {
   for (uint64_t h = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; h < a.n_hub; h += (uint64_t)gridDim.x * blockDim.x) {
@@ -200,20 +233,36 @@ __global__ void combine_hub_kernel(const __grid_constant__ CombineArgs<Prog> a) 
     typename Prog::Acc raw0;
     memcpy(&raw0, &a.out[v], sizeof(raw0));  // the main sweep left its RAW reduction in the value slot
     typename Prog::Wide t = Prog::widen(raw0);
-    // block b has a slot for h while h < N_b; N_b does not increase with b, so h < N_{b+7} means blocks b .. b+7 all
-    // have one: their loads are issued together, the adds keep block order.  Hubs are ordered by in-degree, so the
-    // threads of a warp run about the same number of blocks.
-    uint32_t b = 0;
-    for (; b + 8 <= a.n_blocks && h < a.sg.vbase[b + 8] - a.sg.vbase[b + 7]; b += 8) {
+    // h's bitmap word and lane: the same word for the 32 threads of a warp (the grid stride is a multiple of 32), so
+    // the bitmap and prefix loads are broadcasts, and consecutive hubs with a slot sit at consecutive slots
+    const uint32_t w = (uint32_t)(h >> 5), me = 1u << (h & 31), below = me - 1u;
+    // block b serves h while h < N_b; N_b does not increase with b, so h < N_{b+7} means blocks b .. b+7 all do: their
+    // loads are issued together, the adds keep block order.  Hubs are ordered by in-degree, so the threads of a warp
+    // run about the same number of blocks.
+    auto add8 = [&](uint32_t g) {  // groups g .. g + 7, which all serve h
+      uint32_t bits[8], pre[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        bits[i] = __ldg(a.slot_bits + a.sg.wbase[g + i] + w);
+        pre[i] = __ldg(a.slot_pre + a.sg.wbase[g + i] + w);
+      }
       typename Prog::Acc p[8];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) p[i] = a.partial[a.sg.vbase[b + i] + h];
+      for (int i = 0; i < 8; ++i) p[i] = (bits[i] & me) ? a.partial[pre[i] + __popc(bits[i] & below)] : Prog::identity();
 #pragma unroll
-      for (int i = 0; i < 8; ++i) t = Prog::wcombine(t, Prog::widen(p[i]));
-    }
-    for (; b < a.n_blocks && h < a.sg.vbase[b + 1] - a.sg.vbase[b]; ++b)
-      t = Prog::wcombine(t, Prog::widen(a.partial[a.sg.vbase[b] + h]));
-    for (uint32_t k = a.n_blocks; k < a.n_groups; ++k) t = Prog::wcombine(t, Prog::widen(a.partial[a.sg.vbase[k] + h]));  // cold segments
+      for (int i = 0; i < 8; ++i)
+        if (bits[i] & me) t = Prog::wcombine(t, Prog::widen(p[i]));
+    };
+    auto add = [&](uint32_t g) {
+      const uint32_t bits = __ldg(a.slot_bits + a.sg.wbase[g] + w);
+      if (bits & me) t = Prog::wcombine(t, Prog::widen(a.partial[__ldg(a.slot_pre + a.sg.wbase[g] + w) + __popc(bits & below)]));
+    };
+    uint32_t b = 0;
+    for (; b + 8 <= a.n_blocks && h < a.sg.vbase[b + 8] - a.sg.vbase[b + 7]; b += 8) add8(b);
+    for (; b < a.n_blocks && h < a.sg.vbase[b + 1] - a.sg.vbase[b]; ++b) add(b);
+    uint32_t k = a.n_blocks;  // cold segments: every one serves all hubs
+    for (; k + 8 <= a.n_groups; k += 8) add8(k);
+    for (; k < a.n_groups; ++k) add(k);
     const typename Prog::Vertex oldv = Prog::kNeedsOld ? a.x_nat[a.row_left + v] : typename Prog::Vertex();
     const typename Prog::Vertex nv_ = Prog::update(a.row_left + v, Prog::narrow(t), oldv, a.prm);
     a.out[v] = nv_;

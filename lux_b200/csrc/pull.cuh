@@ -98,6 +98,11 @@ struct PullArgs : PullWeights<Prog::kWeighted> {
   const uint32_t* close_vtx;
 };
 
+// compact slots (panel.cuh): head k of piece t closes slot ps.x + k if lo <= k < end, ps.y = end | lo << 31.  lo = 1
+// only for the first piece of a block, whose first head closes the previous block's last pad.
+constexpr uint32_t kSlotLo = 0x80000000u;
+__device__ __forceinline__ bool piece_slot_real(uint2 ps, uint32_t k) { return k >= (ps.y >> 31) && k < (ps.y & ~kSlotLo); }
+
 template <class Prog>
 __device__ __forceinline__ bool store_raw(const PullArgs<Prog>& a, uint32_t v) {
   if (a.raw_out) return true;
@@ -478,7 +483,7 @@ __global__ void __launch_bounds__(1024) pull_fixup_blocks_kernel(const __grid_co
 }
 
 template <class Prog>
-__global__ void __launch_bounds__(kFixBlock) pull_fixup_apply_kernel(const __grid_constant__ PullArgs<Prog> a) {
+__global__ void __launch_bounds__(kFixBlock) pull_fixup_apply_kernel(const __grid_constant__ PullArgs<Prog> a, const uint2* __restrict__ piece_slot) {
   using Wide = typename Prog::Wide;
   const uint32_t t = blockIdx.x * kFixBlock + threadIdx.x;
   if (t == 0 || t >= a.n_tiles) return;
@@ -488,7 +493,11 @@ __global__ void __launch_bounds__(kFixBlock) pull_fixup_apply_kernel(const __gri
   if (!a.carry_flag[t]) c = Prog::wcombine(a.block_agg[blockIdx.x], c);
   Wide totalw = Prog::wcombine(c, Prog::widen(a.head_partial[t]));
   uint32_t v = i0;
-  if (a.close_vtx) {
+  if (piece_slot) {  // a group stream (seg.cuh): the piece's first head closes its first slot, or a pad
+    const uint2 ps = piece_slot[t];
+    if (!piece_slot_real(ps, 0)) return;
+    v = ps.x;
+  } else if (a.close_vtx) {
     v = a.close_vtx[i0];
     if (v == 0xFFFFFFFFu) return;  // a dummy (padding) vertex
   }
@@ -524,7 +533,8 @@ __device__ __forceinline__ Wide bits_wide(unsigned long long u) {
 }
 
 template <class Prog>
-__global__ void __launch_bounds__(kFixBlock) pull_fixup_fused_kernel(const __grid_constant__ PullArgs<Prog> a, const FixupChain<Prog> ch) {
+__global__ void __launch_bounds__(kFixBlock) pull_fixup_fused_kernel(const __grid_constant__ PullArgs<Prog> a, const FixupChain<Prog> ch,
+                                                                  const uint2* __restrict__ piece_slot) {
   using Wide = typename Prog::Wide;
   __shared__ Wide s_v[kFixBlock / 32];
   __shared__ uint32_t s_f[kFixBlock / 32];
@@ -616,7 +626,11 @@ __global__ void __launch_bounds__(kFixBlock) pull_fixup_fused_kernel(const __gri
   seg_combine<Prog>(cf, c, s_pf, s_pv);
   const Wide totalw = Prog::wcombine(c, Prog::widen(a.head_partial[t]));
   uint32_t vtx = i0;
-  if (a.close_vtx) {
+  if (piece_slot) {
+    const uint2 ps = piece_slot[t];
+    if (!piece_slot_real(ps, 0)) return;
+    vtx = ps.x;
+  } else if (a.close_vtx) {
     vtx = a.close_vtx[i0];
     if (vtx == 0xFFFFFFFFu) return;
   }

@@ -36,7 +36,9 @@ struct PullLayout {
   uint32_t n_tiles = 0;
   FixupScratch fix;
   // flagged stream (seg.cuh): d_src holds the words, d_tile_v the heads before each piece, n_tiles the pieces
-  uint32_t* d_close = nullptr;      // [1 + heads] vertex completed by each head
+  uint32_t* d_close = nullptr;      // [1 + heads] vertex completed by each head (not for the group streams)
+  uint2* d_piece_slot = nullptr;    // group streams: [n_tiles] compact slots closed by each piece (seg.cuh)
+  uint32_t n_slots = 0;             // group streams: slots closed
   uint32_t* d_empty = nullptr;      // vertices without edges in this stream that are not hubs
   uint32_t n_empty = 0;
   uint32_t* d_empty_hub = nullptr;  // ... that are hubs (all their edges moved to the panel)
@@ -290,7 +292,9 @@ struct luxb_graph {
   uint32_t sb_n_hub = 0, sb_n_blocks = 0, sb_n_groups = 0, sb_bs = 0;  // groups: sb_n_blocks panel blocks, then cold segments
   uint32_t* d_hub_vtx = nullptr;
   uint32_t* d_hub_bits = nullptr;
-  uint32_t* d_sb_partial = nullptr;  // [vbase[sb_n_groups]] raw reductions of every (group, hub) slot (4-byte Acc)
+  uint32_t* d_sb_partial = nullptr;  // [slots] raw reductions of every (group, hub) pair with edges (4-byte Acc)
+  uint32_t* d_slot_bits = nullptr;   // [wbase[sb_n_groups]] which (group, hub) pairs have a slot (panel.cuh)
+  uint32_t* d_slot_pre = nullptr;    // [wbase[sb_n_groups] + 1] slots before each bitmap word
   luxb::SplitGroups sb_groups{};
   uint32_t sb_super_end[luxb::kPanelMaxBlocks]{};
   // cold-hub stream (PageRank, one rank): cold source segment x hub destination, gathered through L1 from an L2-sized

@@ -7,11 +7,13 @@
 //   * the edge stream carries its own structure: the top bit of an edge word says "this edge starts a new destination
 //     vertex" (head flag); the rest is the gather id (31 bits: hot-packed id; panel: 15-bit offset into the block's table);
 //   * close_vtx[j] = the vertex whose in-edge list ENDS where head j begins (one u32 per non-empty vertex instead of
-//     one row_end word per vertex; vertices without in-edges are handled by empties_kernel);
+//     one row_end word per vertex; vertices without in-edges are handled by empties_kernel).  The group streams of the
+//     split (panel, cold-hub; panel.cuh) close their slots in slot order, so they keep no such list: per piece t,
+//     piece_slot[t] = (slot0, real range) and head k of the piece closes slot slot0 + k (kSlots);
 //   * a warp owns a PIECE of kRounds x 32 x kV consecutive edges; per round each lane loads kV (8 or 16) consecutive words
 //     with 128-bit shared-memory loads, issues its kV gathers, reduces them serially up to the head flags, and one
 //     segmented warp-shuffle scan stitches the lanes; completed sums are staged in shared memory and written by a
-//     lane-strided pass (update() + coalesced close_vtx loads).  The running carry across rounds is kept in the
+//     lane-strided pass (update() + coalesced close_vtx loads, or consecutive slots).  The running carry across rounds is kept in the
 //     program's wide type (fp64 for PageRank);
 //   * the stream is padded with head-flagged dummy edges to whole stages, so the kernel has no bounds checks;
 //   * pieces are claimed stage by stage from a global counter by a producer warp that streams the words with ONE TMA
@@ -36,6 +38,7 @@ struct SegShape {
   static constexpr int kStages = kStages_;
   static constexpr int kRounds = kRounds_;
   static constexpr bool kPanel = kPanel_;
+  static constexpr bool kSlots = kPanel_;                 // heads close compact slots (piece_slot), not close_vtx
   static constexpr int kTab = kTab_;                      // shared-memory table (values); 0 for the L1 sweep
   static constexpr int kV = kV_;                          // consecutive edges per lane and round (8 or 16)
   static constexpr int kRound = 32 * kV;                  // edges per warp round
@@ -52,6 +55,12 @@ struct SegShape {
   static_assert(kV == 8 || kV == 16, "a lane reads its words with 128-bit loads");
 };
 
+// a main (L1-gather) shape sweeping a group stream: the cold-hub stream
+template <class Base>
+struct SlotShape : Base {
+  static constexpr bool kSlots = true;
+};
+
 template <class Prog>
 struct SegArgs {
   PullArgs<Prog> p;          // out / update() parameters / hub_bits / raw_out / head+tail partials / tile_v / close_vtx
@@ -61,6 +70,8 @@ struct SegArgs {
   // panel only
   uint32_t bs, n_blocks;
   uint32_t super_end[kPanelMaxBlocks];
+  // group streams (Shape::kSlots): [n_tiles] slot0 and real range of every piece, in place of p.close_vtx
+  const uint2* piece_slot;
 };
 
 template <class Prog, class Shape>
@@ -69,7 +80,7 @@ __global__ void __launch_bounds__(Shape::kThreads, Shape::kPanel ? 1 : 2) seg_ti
   using Vertex = typename Prog::Vertex;
   using Wide = typename Prog::Wide;
   constexpr int kStages = Shape::kStages, kWarps = Shape::kWarps, kRounds = Shape::kRounds, kV = Shape::kV;
-  constexpr bool kPanel = Shape::kPanel;
+  constexpr bool kPanel = Shape::kPanel, kSlots = Shape::kSlots;
   static_assert(sizeof(Acc) == 4 && sizeof(Vertex) == 4, "4-byte vertex values");
 
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -171,6 +182,12 @@ __global__ void __launch_bounds__(Shape::kThreads, Shape::kPanel ? 1 : 2) seg_ti
     const uint32_t t = T * kWarps + warp;   // piece index
     const uint32_t jbase = hdr[2 + warp];   // heads before this piece
     const unsigned char* P = w_buf + (size_t)s * Shape::kStageBytes + (size_t)warp * Shape::kPiece * Shape::kWordBytes;
+    uint32_t slot0 = 0, slot_end = 0;  // kSlots: head k (>= 1: head 0 is the fix-up's) closes slot slot0 + k if k < slot_end
+    if constexpr (kSlots) {
+      const uint2 ps = __ldg(a.piece_slot + t);
+      slot0 = ps.x;
+      slot_end = ps.y & ~kSlotLo;
+    }
 
     Wide carry = Prog::widen(Prog::identity());  // warp-uniform: reduction of the edges since the last head
     bool seen = false;                           // a head has been met in this piece
@@ -237,12 +254,14 @@ __global__ void __launch_bounds__(Shape::kThreads, Shape::kPanel ? 1 : 2) seg_ti
       const uint32_t excl = incl - cnt;
       const uint32_t n_round = __shfl_sync(0xffffffffu, incl, 31);
       // the vertices this round completes: request their ids now, they are needed only after the reduction below
-      constexpr int kPre = kV / 4;  // covers the typical number of completions per round (one per ~8 edges)
+      constexpr int kPre = kSlots ? 1 : kV / 4;  // covers the typical number of completions per round (one per ~8 edges)
       uint32_t vpre[kPre];
+      if constexpr (!kSlots) {
 #pragma unroll
-      for (int q = 0; q < kPre; ++q) {
-        const uint32_t li = lane + 32 * q;
-        vpre[q] = li < n_round ? __ldg(a.p.close_vtx + jbase + n_closed + li) : kDummyVtx;
+        for (int q = 0; q < kPre; ++q) {
+          const uint32_t li = lane + 32 * q;
+          vpre[q] = li < n_round ? __ldg(a.p.close_vtx + jbase + n_closed + li) : kDummyVtx;
+        }
       }
       // ---- serial segmented reduction inside the lane ----
       Acc run = Prog::identity(), first_val = Prog::identity();
@@ -305,12 +324,22 @@ __global__ void __launch_bounds__(Shape::kThreads, Shape::kPanel ? 1 : 2) seg_ti
         if (kPanel) a.p.out[v] = sums[li];   // raw partial sum of a (block, hub) pair; combine_hub_kernel finishes the hub
         else store_vertex<Prog>(a.p, v, sums[li]);
       };
+      if constexpr (kSlots) {
+        for (uint32_t li = lane; li < n_round; li += 32) {
+          const uint32_t k = n_closed + li;
+          if (li == 0 && defer_first) continue;
+          if (k >= slot_end) break;  // the rest are pads
+          if (kPanel) a.p.out[slot0 + k] = sums[li];
+          else store_vertex<Prog>(a.p, slot0 + k, sums[li]);
+        }
+      } else {
 #pragma unroll
-      for (int q = 0; q < kPre; ++q) {
-        const uint32_t li = lane + 32 * q;
-        if (li < n_round) finish(li, vpre[q]);
+        for (int q = 0; q < kPre; ++q) {
+          const uint32_t li = lane + 32 * q;
+          if (li < n_round) finish(li, vpre[q]);
+        }
+        for (uint32_t li = lane + 32 * kPre; li < n_round; li += 32) finish(li, __ldg(a.p.close_vtx + jbase + n_closed + li));
       }
-      for (uint32_t li = lane + 32 * kPre; li < n_round; li += 32) finish(li, __ldg(a.p.close_vtx + jbase + n_closed + li));
       n_closed += n_round;
       __syncwarp();
     }
@@ -320,7 +349,7 @@ __global__ void __launch_bounds__(Shape::kThreads, Shape::kPanel ? 1 : 2) seg_ti
 
 // ---- one-time construction of a flagged stream ---------------------------------------------------------------------
 // one thread per "vertex" of a CSC (row_end inclusive): non-empty ones mark their first edge word and register
-// themselves in the close list (shifted by one: entry j+1 holds the vertex that owns head j).
+// themselves in the close list, if there is one (shifted by one: entry j+1 holds the vertex that owns head j).
 struct StreamBlocks {            // vertices [vfirst[b], vfirst[b+1]) live in block b (main stream: one block)
   uint32_t n_blocks;
   uint32_t vfirst[kPanelMaxBlocks + 1];
@@ -348,14 +377,14 @@ __global__ void nonempty_flag_kernel(const uint64_t* __restrict__ row_end, uint3
 template <class Word>
 __global__ void stream_heads_kernel(const uint64_t* __restrict__ row_end, uint32_t n_vtx, const uint32_t* __restrict__ flag,
                                     const uint32_t* __restrict__ segrank, const __grid_constant__ StreamBlocks sb,
-                                    Word* __restrict__ words, uint32_t* __restrict__ close_list, uint32_t vtx_offset) {
+                                    Word* __restrict__ words, uint32_t* __restrict__ close_list) {
   constexpr Word kHead = (Word)1 << (sizeof(Word) * 8 - 1);
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_vtx; i += (uint64_t)gridDim.x * blockDim.x) {
     if (!flag[i]) continue;
     const uint32_t b = find_block(sb.vfirst, sb.n_blocks, i);
     const uint64_t begin = i == 0 ? 0 : row_end[i - 1];
     words[begin - sb.ebase[b] + sb.wbase[b]] |= kHead;
-    close_list[1 + (uint64_t)segrank[i] + sb.hshift[b]] = (uint32_t)i + vtx_offset;
+    if (close_list) close_list[1 + (uint64_t)segrank[i] + sb.hshift[b]] = (uint32_t)i;
   }
 }
 
@@ -388,6 +417,24 @@ __global__ void piece_heads_kernel(const Word* __restrict__ words, uint32_t n_pi
 #pragma unroll
     for (int off = 16; off; off >>= 1) c += __shfl_xor_sync(0xffffffffu, c, off);
     if (lane == 0) cnt[t] = c;
+  }
+}
+
+// compact slots of a group stream (its "vertices" are the (group, hub) pairs; non-empty ones are slots slot_base +
+// segrank): piece t lies in one block b (blocks are padded to whole stages).  Block b's heads start at
+// hb = segrank[vfirst[b]] + hshift[b]; head hb closes the previous block's last pad (a dummy), heads hb + 1 ..
+// hb + n_b close the block's n_b slots in order, the heads after them close pads.  So head J of block b closes slot
+// slot_base + J - 1 - hshift[b] when hb < J <= hb + n_b: piece t's real heads are one run.
+__global__ void piece_slot_kernel(const uint32_t* __restrict__ tile_v, uint32_t n_pieces, uint32_t piece, const uint32_t* __restrict__ segrank,
+                                  const __grid_constant__ StreamBlocks sb, uint32_t slot_base, uint2* __restrict__ piece_slot) {
+  for (uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n_pieces; t += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t b = find_block(sb.wbase, sb.n_blocks, t * piece);
+    const int64_t r0 = segrank[sb.vfirst[b]], r1 = segrank[sb.vfirst[b + 1]];
+    const int64_t hb = r0 + (int64_t)sb.hshift[b];
+    const int64_t i0 = tile_v[t], i1 = tile_v[t + 1];
+    const int64_t last = i1 < hb + 1 + (r1 - r0) ? i1 : hb + 1 + (r1 - r0);  // one past the piece's last real head
+    const int64_t end = last > i0 ? last - i0 : 0;
+    piece_slot[t] = make_uint2((uint32_t)((int64_t)slot_base + i0 - 1 - (int64_t)sb.hshift[b]), (uint32_t)end | (i0 == hb ? kSlotLo : 0u));
   }
 }
 
