@@ -56,7 +56,10 @@ static_assert(kNumApps == LUXB_TRUSS + 1, "one row per luxb_app");
 // the handle's app (its config passed check_config at open)
 static const AppInfo& app_of(const luxb_graph* g) { return kApps[g->cfg.app]; }
 
-static const char* const kPhaseName[12] = {"pull_tile", "fixup", "refresh", "rechunk", "barrier", "panel", "combine", "pack+push", "pull/bcast", "cold_hub", "bc_sigma", "bc_delta"};
+// 0 .. 11: phases of the compute stream (the concurrent sweep's side stream adds to pull_tile, fixup and cold_hub);
+// 12 .. 14: the concurrent sweep's main kernel on the panel's SMs, the wait for the side stream, the whole overlapped region
+static const char* const kPhaseName[15] = {"pull_tile", "fixup", "refresh", "rechunk", "barrier", "panel", "combine", "pack+push",
+                                           "pull/bcast", "cold_hub", "bc_sigma", "bc_delta", "main_join", "join_wait", "overlap"};
 static void pt_mark(luxb_graph* g, int tag) {
   PhaseTimer& pt = g->pt;
   if (!pt.on) return;
@@ -65,6 +68,19 @@ static void pt_mark(luxb_graph* g, int tag) {
   cudaEventRecord(e, g->stream);
   pt.ev.push_back(e);
   pt.tag.push_back(tag);
+}
+// an event on stream st for pt_span: its index, or -1 when the timer is off
+static int pt_event(luxb_graph* g, cudaStream_t st) {
+  PhaseTimer& pt = g->pt;
+  if (!pt.on) return -1;
+  cudaEvent_t e;
+  cudaEventCreate(&e);
+  cudaEventRecord(e, st);
+  pt.span_ev.push_back(e);
+  return (int)pt.span_ev.size() - 1;
+}
+static void pt_span(luxb_graph* g, int tag, int begin, int end) {
+  if (begin >= 0) g->pt.spans.push_back({begin, end, tag});
 }
 static void pt_print(luxb_graph* g) {
   if (g->pt.on && g->pt.cnt) {
@@ -77,6 +93,10 @@ static void pt_print(luxb_graph* g) {
       n += snprintf(line + n, sizeof(line) - n, " %s %.3f ms;", kPhaseName[k], g->pt.sum[k] / g->pt.cnt);
       sum += g->pt.sum[k] / g->pt.cnt;
     }
+    if (!bc && g->pt.sum[14] > 0) {  // concurrent sweep: the phases above overlap, the compute stream's total is the time
+      for (int k = 12; k < 15; ++k) n += snprintf(line + n, sizeof(line) - n, " %s %.3f ms;", kPhaseName[k], g->pt.sum[k] / g->pt.cnt);
+      sum = g->pt.chain / g->pt.cnt;
+    }
     snprintf(line + n, sizeof(line) - n, " sum %.3f ms\n", sum);
     fputs(line, stderr);  // one write per rank: the ranks' lines do not interleave
   }
@@ -85,18 +105,29 @@ static void pt_print(luxb_graph* g) {
 static void pt_flush(luxb_graph* g) {
   PhaseTimer& pt = g->pt;
   if (!pt.on || pt.ev.empty()) return;
-  cudaStreamSynchronize(g->stream);
+  cudaStreamSynchronize(g->stream);  // the side stream joins the compute stream before every sweep ends
+  // one PageRank iteration (its pull sweep), or one BC source (its σ sweep: the BFS's own pull sweeps also mark tag 0)
+  const int count_tag = app_of(g).entry == kBcRun ? 10 : 0;
   for (size_t i = 1; i < pt.ev.size(); ++i) {
     if (pt.tag[i] < 0) continue;
     float ms = 0;
     cudaEventElapsedTime(&ms, pt.ev[i - 1], pt.ev[i]);
     pt.sum[pt.tag[i]] += ms;
-    // one PageRank iteration (its pull sweep), or one BC source (its σ sweep: the BFS's own pull sweeps also mark tag 0)
-    if (pt.tag[i] == (app_of(g).entry == kBcRun ? 10 : 0)) pt.cnt++;
+    pt.chain += ms;
+    if (pt.tag[i] == count_tag) pt.cnt++;
+  }
+  for (const PhaseTimer::Span& s : pt.spans) {
+    float ms = 0;
+    cudaEventElapsedTime(&ms, pt.span_ev[s.begin], pt.span_ev[s.end]);
+    pt.sum[s.tag] += ms;
+    if (s.tag == count_tag) pt.cnt++;
   }
   for (cudaEvent_t e : pt.ev) cudaEventDestroy(e);
+  for (cudaEvent_t e : pt.span_ev) cudaEventDestroy(e);
   pt.ev.clear();
   pt.tag.clear();
+  pt.span_ev.clear();
+  pt.spans.clear();
 }
 
 
@@ -1002,6 +1033,7 @@ static int set_l2_persisting_window(luxb_graph* g, void* base, size_t bytes) {
   attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
   attr.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
   LUXB_CUDA(cudaStreamSetAttribute(g->stream, cudaStreamAttributeAccessPolicyWindow, &attr));
+  if (g->stream_b) LUXB_CUDA(cudaStreamSetAttribute(g->stream_b, cudaStreamAttributeAccessPolicyWindow, &attr));
   if (g->cfg.verbose) printf("L2 persisting window: %zu bytes (device max persisting %d, max window %d)\n", persist, max_persist, max_window);
   return 0;
 }
@@ -1177,6 +1209,11 @@ static int build_gather_side(luxb_graph* g, bool compact_cold, bool streams) {
   if (g->P > 1) LUXB_NCCL(nccl().AllReduce(g->d_deg, g->d_deg, g->nv, ncclUint32, ncclSum, g->comm, g->stream));
   LUXB_TRY(build_hot_layout(g, compact_cold));
   if (streams) LUXB_TRY(build_seg_sweep(g));
+  if (g->sb_on && g->P == 1) {  // the side stream of the concurrent split sweep (sweep_seg)
+    LUXB_CUDA(cudaStreamCreateWithFlags(&g->stream_b, cudaStreamNonBlocking));
+    LUXB_CUDA(cudaEventCreateWithFlags(&g->ev_fork, cudaEventDisableTiming));
+    LUXB_CUDA(cudaEventCreateWithFlags(&g->ev_join, cudaEventDisableTiming));
+  }
   if (g->hot_n) {
     const uint64_t z_len = (uint64_t)g->hot_n + (g->cold_z ? g->cold_n : 0) + 65536;
     LUXB_TRY(gmalloc(g, (uint32_t**)&g->d_hot, z_len));
@@ -1365,14 +1402,16 @@ static void fill_fixup_args(PullArgs<Prog>& a, const FixupScratch& f) {
   a.block_flag = f.d_block_flag;
 }
 
-// f is the sweep's own scratch (the fused fix-up keeps its launch epoch there)
+// f is the sweep's own scratch (the fused fix-up keeps its launch epoch there); st: the stream of the swept kernel
 template <class Prog>
-static int launch_fixup(luxb_graph* g, const PullArgs<Prog>& a, FixupScratch& f, const uint2* piece_slot = nullptr) {
+static int launch_fixup(luxb_graph* g, const PullArgs<Prog>& a, FixupScratch& f, const uint2* piece_slot = nullptr,
+                        cudaStream_t st = nullptr) {
   if (a.n_tiles <= 1) return 0;
+  if (!st) st = g->stream;
   if (g->fused_fixup) {
     if (!f.d_chain) {
       LUXB_TRY(gmalloc(g, &f.d_chain, 4ull * f.n_fix_blocks + 4));  // values, status words, [4 n] = ticket counter
-      LUXB_CUDA(cudaMemsetAsync(f.d_chain, 0, (4ull * f.n_fix_blocks + 4) * 8, g->stream));
+      LUXB_CUDA(cudaMemsetAsync(f.d_chain, 0, (4ull * f.n_fix_blocks + 4) * 8, st));
       f.chain_epoch = 0;
     }
     FixupChain<Prog> ch;
@@ -1382,17 +1421,17 @@ static int launch_fixup(luxb_graph* g, const PullArgs<Prog>& a, FixupScratch& f,
     ch.n_blocks = f.n_fix_blocks;
     ch.epoch = ++f.chain_epoch;
     if (f.chain_epoch >= 0x3FFFFFF0u) {  // 30-bit epochs: start over with a clean status array
-      LUXB_CUDA(cudaMemsetAsync(f.d_chain, 0, (4ull * f.n_fix_blocks + 4) * 8, g->stream));
+      LUXB_CUDA(cudaMemsetAsync(f.d_chain, 0, (4ull * f.n_fix_blocks + 4) * 8, st));
       f.chain_epoch = ch.epoch = 1;
     }
-    pull_fixup_fused_kernel<Prog><<<f.n_fix_blocks, kFixBlock, 0, g->stream>>>(a, ch, piece_slot);
+    pull_fixup_fused_kernel<Prog><<<f.n_fix_blocks, kFixBlock, 0, st>>>(a, ch, piece_slot);
     LUXB_CUDA(cudaGetLastError());
     g->stats.kernel_launches++;
     return 0;
   }
-  pull_fixup_scan_kernel<Prog><<<f.n_fix_blocks, kFixBlock, 0, g->stream>>>(a);
-  pull_fixup_blocks_kernel<Prog><<<1, 1024, 0, g->stream>>>(a, f.n_fix_blocks);
-  pull_fixup_apply_kernel<Prog><<<f.n_fix_blocks, kFixBlock, 0, g->stream>>>(a, piece_slot);
+  pull_fixup_scan_kernel<Prog><<<f.n_fix_blocks, kFixBlock, 0, st>>>(a);
+  pull_fixup_blocks_kernel<Prog><<<1, 1024, 0, st>>>(a, f.n_fix_blocks);
+  pull_fixup_apply_kernel<Prog><<<f.n_fix_blocks, kFixBlock, 0, st>>>(a, piece_slot);
   LUXB_CUDA(cudaGetLastError());
   g->stats.kernel_launches += 3;
   return 0;
@@ -1492,6 +1531,7 @@ static void resolve_sweep_settings(SweepSettings& s) {
   s.hot_mb = env_double("LUXB_HOT_MB", s.hot_mb);
   s.l2_persist = env_int("LUXB_L2_PERSIST", 1) != 0;
   s.l2_window_mb = env_double("LUXB_L2_WINDOW_MB", s.l2_window_mb);
+  s.panel_sms = std::max(0, env_int("LUXB_PANEL_SMS", s.panel_sms));
 }
 
 extern "C++" {
@@ -1926,8 +1966,9 @@ static int build_seg_sweep(luxb_graph* g) {
 }
 
 extern "C++" {
+// sms: the SMs whose worth of CTAs (ctas_per_sm each) the grid holds; st: the stream
 template <class Prog, class Shape>
-static int launch_seg_shape(luxb_graph* g, const SegArgs<Prog>& a, int ctas_per_sm) {
+static int launch_seg_shape(luxb_graph* g, const SegArgs<Prog>& a, int sms, int ctas_per_sm, cudaStream_t st) {
   auto kern = seg_tile_kernel<Prog, Shape>;
   // The panel kernel holds one persistent CTA with ~all of the shared memory on every SM it runs on; when the cold half
   // of the exchange is in flight on the second stream (several ranks), a few SMs are left to NCCL's channel CTAs —
@@ -1936,19 +1977,16 @@ static int launch_seg_shape(luxb_graph* g, const SegArgs<Prog>& a, int ctas_per_
   LUXB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Shape::kSmemBytes));
   int carve_pct = (int)std::min<size_t>(100, (ctas_per_sm * (Shape::kSmemBytes + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024));
   LUXB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, carve_pct));
-  const uint32_t grid = (uint32_t)std::min<uint64_t>((uint64_t)std::max(g->num_sms - reserve, 1) * ctas_per_sm, a.n_stages);
-  kern<<<grid, Shape::kThreads, Shape::kSmemBytes, g->stream>>>(a);
+  const uint32_t grid = (uint32_t)std::min<uint64_t>((uint64_t)std::max(std::min(sms, g->num_sms - reserve), 1) * ctas_per_sm, a.n_stages);
+  kern<<<grid, Shape::kThreads, Shape::kSmemBytes, st>>>(a);
   LUXB_CUDA(cudaGetLastError());
   return 0;
 }
 
-// one flagged stream L (seg.cuh): the seg kernel in shape `shape` of the panel (kPanel) or the main family, then its
-// fix-up.  The caller has set a's stream-specific fields; L's own arrays are filled here.  counter_slot: the stream's
-// tile counter in d_counters; tag: the phase-timer slot of the kernel.  kSlots: a main shape over a group stream
-// (the cold-hub stream; the panel always is one).
-template <bool kPanel, class Prog, bool kSlots = kPanel>
-static int launch_seg_stream(luxb_graph* g, PullLayout& L, SegArgs<Prog>& a, int shape, int ctas_per_sm, int counter_slot, int tag,
-                             const char* name) {
+// the fields of a that come from the flagged stream L (seg.cuh); counter_slot: the stream's tile counter in d_counters
+// (main 2, panel 4, cold-hub 5), which sweep_seg zeroes before the sweep.  The caller sets the stream-specific fields.
+template <class Prog>
+static void seg_stream_args(luxb_graph* g, PullLayout& L, SegArgs<Prog>& a, int counter_slot) {
   a.p.tile_v = L.d_tile_v;
   a.p.n_tiles = L.n_tiles;
   fill_fixup_args(a.p, L.fix);
@@ -1957,11 +1995,18 @@ static int launch_seg_stream(luxb_graph* g, PullLayout& L, SegArgs<Prog>& a, int
   a.words = L.d_src;
   a.n_stages = L.n_stages;
   a.tile_counter = reinterpret_cast<uint32_t*>(g->d_counters + counter_slot);
-  LUXB_CUDA(cudaMemsetAsync(a.tile_counter, 0, 4, g->stream));
+}
+
+// the seg kernel of one flagged stream in shape `shape` of the panel (kPanel) or the main family, on `sms` SMs' worth of
+// CTAs, on stream st; its fix-up is the caller's.  kSlots: a main shape over a group stream (the cold-hub stream; the
+// panel always is one).
+template <bool kPanel, class Prog, bool kSlots = kPanel>
+static int launch_seg_kernel(luxb_graph* g, const SegArgs<Prog>& a, int shape, int sms, int ctas_per_sm, cudaStream_t st,
+                             const char* name) {
 #define LUXB_CASE_MSHAPE(id, warps, stages, rounds) \
-  case id: LUXB_TRY((launch_seg_shape<Prog, std::conditional_t<kSlots, SlotShape<SegMain##id>, SegMain##id>>(g, a, ctas_per_sm))); break;
+  case id: LUXB_TRY((launch_seg_shape<Prog, std::conditional_t<kSlots, SlotShape<SegMain##id>, SegMain##id>>(g, a, sms, ctas_per_sm, st))); break;
 #define LUXB_CASE_PSHAPE(id, warps, stages, rounds, tab, v) \
-  case id: LUXB_TRY((launch_seg_shape<Prog, SegPanel##id>(g, a, ctas_per_sm))); break;
+  case id: LUXB_TRY((launch_seg_shape<Prog, SegPanel##id>(g, a, sms, ctas_per_sm, st))); break;
   if constexpr (kPanel) {
     switch (shape) {
       LUXB_SEG_PANEL_SHAPES(LUXB_CASE_PSHAPE)
@@ -1974,18 +2019,23 @@ static int launch_seg_stream(luxb_graph* g, PullLayout& L, SegArgs<Prog>& a, int
     }
   }
   g->stats.kernel_launches++;
+  return 0;
+}
+
+// one flagged stream L swept on all SMs (g->stream), then its fix-up; tag: the phase-timer slot of the kernel
+template <bool kPanel, class Prog, bool kSlots = kPanel>
+static int launch_seg_stream(luxb_graph* g, PullLayout& L, const SegArgs<Prog>& a, int shape, int ctas_per_sm, int tag, const char* name) {
+  LUXB_TRY((launch_seg_kernel<kPanel, Prog, kSlots>(g, a, shape, g->num_sms, ctas_per_sm, g->stream, name)));
   pt_mark(g, tag);
   return launch_fixup(g, a.p, L.fix, L.d_piece_slot);
 }
 }  // extern "C++"
 
 extern "C++" {
-// main (L1) stream of a pull sweep: seg kernel + fix-up + vertices without in-edges.
-// out_buffer >= 0 (PageRank): index of the value buffer written, for the once-per-buffer constants of edge-less vertices;
-// < 0 (labels): `out_local` already holds the old values, edge-less vertices keep them.
+// arguments of the main (L1) stream of a pull sweep
 template <class Prog>
-static int launch_seg_main(luxb_graph* g, PullLayout& L, const typename Prog::Vertex* x_nat, const typename Prog::Vertex* x_cold,
-                           typename Prog::Vertex* out_local, int out_buffer, const typename Prog::Params& prm, const uint32_t* hub_bits) {
+static SegArgs<Prog> seg_main_args(luxb_graph* g, PullLayout& L, const typename Prog::Vertex* x_nat, const typename Prog::Vertex* x_cold,
+                                   typename Prog::Vertex* out_local, const typename Prog::Params& prm, const uint32_t* hub_bits) {
   SegArgs<Prog> a{};
   a.p.n_part = L.n_vtx;
   a.p.row_left = g->row_left;
@@ -1997,32 +2047,48 @@ static int launch_seg_main(luxb_graph* g, PullLayout& L, const typename Prog::Ve
   a.p.prm = prm;
   a.p.hub_bits = hub_bits;
   a.p.l2_hints = g->l2_hints;
-  LUXB_TRY(wait_cold_exchange(g));
-  LUXB_TRY((launch_seg_stream<false, Prog>(g, L, a, g->sweep.main_shape, g->pull_ctas, 2, 0, "seg")));
-  // vertices without in-edges in this stream.  PageRank: update(identity) is a constant -> written once per value
-  // buffer.  Hubs among them need the raw identity every sweep (the combine overwrites it).
+  seg_stream_args(g, L, a, 2);
+  return a;
+}
+
+// after the main stream's fix-up: its vertices without in-edges.
+// out_buffer >= 0 (PageRank): index of the value buffer written, for the once-per-buffer constants of edge-less vertices;
+// < 0 (labels): `out_local` already holds the old values, edge-less vertices keep them.
+template <class Prog>
+static int launch_seg_empties(luxb_graph* g, PullLayout& L, const PullArgs<Prog>& p, int out_buffer) {
+  // PageRank: update(identity) is a constant -> written once per value buffer.  Hubs among them need the raw identity
+  // every sweep (the combine overwrites it).
   if (out_buffer >= 0 && L.n_empty && !g->empties_done[out_buffer]) {
-    empties_kernel<Prog><<<grid_for(L.n_empty, 256, g->num_sms * 8), 256, 0, g->stream>>>(a.p, L.d_empty, L.n_empty);
+    empties_kernel<Prog><<<grid_for(L.n_empty, 256, g->num_sms * 8), 256, 0, g->stream>>>(p, L.d_empty, L.n_empty);
     g->empties_done[out_buffer] = true;
     g->stats.kernel_launches++;
   }
   if (L.n_empty_hub) {
-    empties_kernel<Prog><<<grid_for(L.n_empty_hub, 256, g->num_sms * 8), 256, 0, g->stream>>>(a.p, L.d_empty_hub, L.n_empty_hub);
+    empties_kernel<Prog><<<grid_for(L.n_empty_hub, 256, g->num_sms * 8), 256, 0, g->stream>>>(p, L.d_empty_hub, L.n_empty_hub);
     g->stats.kernel_launches++;
   }
   LUXB_CUDA(cudaGetLastError());
-  pt_mark(g, 1);
   return 0;
 }
 
-// one pull sweep = [panel stream (shared-memory gathers) +] main stream (L1 gathers) [+ hub combine]
+// one pull sweep = [panel stream (shared-memory gathers) +] [cold-hub stream +] main stream (L1 gathers) [+ hub combine].
+// The panel kernel is bound by shared-memory gathers and instruction issue on each SM; the cold-hub and main kernels
+// by the rate at which the L2 serves random sector requests, a limit of the whole device rather than of each SM.  So
+// on one rank (stream_b exists) with 0 < S = LUXB_PANEL_SMS < SMs they run at the same time:
+//   g->stream:  panel kernel on S SMs -> panel fix-up -> main kernel again, S SMs' worth of CTAs ("join launch") -> join
+//   stream_b:   cold-hub kernel on the other SMs -> cold-hub fix-up -> main kernel on the other SMs
+// The two main launches share one SegArgs and so one tile counter: the join launch's CTAs claim whatever main stages
+// are left once the panel is done, and every stage is still claimed exactly once, so the pieces, partials and fix-ups
+// are those of the serial order and every value is bit for bit the same.  A panel CTA takes ~all of an SM's shared
+// memory, so the side stream's CTAs cannot land on the panel's SMs while it runs; the panel is launched first so that
+// its CTAs are dispatched before them.  Several ranks keep the serial order (stream2 carries the overlapped exchange).
 template <class Prog>
 static int sweep_seg(luxb_graph* g, const typename Prog::Vertex* x_nat, const typename Prog::Vertex* x_cold, typename Prog::Vertex* out_local,
                      int out_buffer, const typename Prog::Params& prm) {
   using Acc = typename Prog::Acc;
-  LUXB_TRY(kt_begin(g));
+  constexpr bool kColdHub = std::is_same<Prog, PageRankProgram>::value;
+  SegArgs<Prog> pa{}, ca{};
   if (g->sb_on) {
-    SegArgs<Prog> pa{};
     pa.p.x_hot = reinterpret_cast<const typename Prog::Vertex*>(g->d_hot);
     pa.p.out = reinterpret_cast<typename Prog::Vertex*>(g->d_sb_partial);
     pa.p.raw_out = 1;
@@ -2030,15 +2096,13 @@ static int sweep_seg(luxb_graph* g, const typename Prog::Vertex* x_nat, const ty
     pa.bs = g->sb_bs;
     pa.n_blocks = g->sb_n_blocks;
     for (uint32_t b = 0; b < g->sb_n_blocks; ++b) pa.super_end[b] = g->sb_super_end[b];
-    LUXB_TRY((launch_seg_stream<true, Prog>(g, g->sb_panel, pa, g->sweep.panel_shape, 1, 4, 5, "panel")));
-    pt_mark(g, 1);
+    seg_stream_args(g, g->sb_panel, pa, 4);
   }
   if (g->cs_on) {
     // cold-hub stream: raw partial per (cold segment, hub) slot; its gathers all index the compact cold values, which it
     // loads with evict_normal (l2_hints = 0): the current segment is meant to stay in L2 while the SMs sweep it.  Only
     // PageRank builds it (the compact cold copy is PageRank's), so only PageRank instantiates its kernels.
-    if constexpr (std::is_same<Prog, PageRankProgram>::value) {
-      SegArgs<Prog> ca{};
+    if constexpr (kColdHub) {
       ca.p.x_old = x_cold;
       ca.p.x_hot = reinterpret_cast<const typename Prog::Vertex*>(g->d_hot);
       ca.p.hot_n = g->hot_n;
@@ -2046,30 +2110,80 @@ static int sweep_seg(luxb_graph* g, const typename Prog::Vertex* x_nat, const ty
       ca.p.raw_out = 1;
       ca.p.l2_hints = 0;
       ca.p.prm = prm;
-      LUXB_TRY((launch_seg_stream<false, Prog, true>(g, g->sb_cold, ca, g->sweep.cs_shape, g->pull_ctas, 4, 9, "cold-hub")));
-      pt_mark(g, 1);
+      seg_stream_args(g, g->sb_cold, ca, 5);
     } else {
       set_error("the cold-hub stream is built for PageRank only");
       return LUXB_ERR_STATE;
     }
   }
-  LUXB_TRY((launch_seg_main<Prog>(g, g->sb_main, x_nat, x_cold, out_local, out_buffer, prm, g->sb_on ? g->d_hub_bits : nullptr)));
+  const SegArgs<Prog> ma = seg_main_args<Prog>(g, g->sb_main, x_nat, x_cold, out_local, prm, g->sb_on ? g->d_hub_bits : nullptr);
+  const int S = g->sweep.panel_sms;
+  const bool beside = g->stream_b && S > 0 && S < g->num_sms;
+  LUXB_TRY(kt_begin(g));
+  LUXB_CUDA(cudaMemsetAsync(g->d_counters + 2, 0, 4, g->stream));
+  if (g->sb_on) LUXB_CUDA(cudaMemsetAsync(g->d_counters + 4, 0, 16, g->stream));
+  if (beside) {
+    cudaStream_t sb = g->stream_b;
+    LUXB_CUDA(cudaEventRecord(g->ev_fork, g->stream));
+    const int t_fork = pt_event(g, g->stream);
+    LUXB_TRY((launch_seg_kernel<true, Prog>(g, pa, g->sweep.panel_shape, S, 1, g->stream, "panel")));
+    pt_mark(g, 5);
+    LUXB_CUDA(cudaStreamWaitEvent(sb, g->ev_fork, 0));
+    int t = pt_event(g, sb);
+    if constexpr (kColdHub) {
+      if (g->cs_on) {
+        LUXB_TRY((launch_seg_kernel<false, Prog, true>(g, ca, g->sweep.cs_shape, g->num_sms - S, g->pull_ctas, sb, "cold-hub")));
+        const int t_cold = pt_event(g, sb);
+        pt_span(g, 9, t, t_cold);
+        LUXB_TRY(launch_fixup(g, ca.p, g->sb_cold.fix, g->sb_cold.d_piece_slot, sb));
+        t = pt_event(g, sb);
+        pt_span(g, 1, t_cold, t);
+      }
+    }
+    LUXB_TRY((launch_seg_kernel<false, Prog>(g, ma, g->sweep.main_shape, g->num_sms - S, g->pull_ctas, sb, "seg")));
+    pt_span(g, 0, t, pt_event(g, sb));
+    LUXB_CUDA(cudaEventRecord(g->ev_join, sb));
+    LUXB_TRY(launch_fixup(g, pa.p, g->sb_panel.fix, g->sb_panel.d_piece_slot));
+    pt_mark(g, 1);
+    LUXB_TRY((launch_seg_kernel<false, Prog>(g, ma, g->sweep.main_shape, S, g->pull_ctas, g->stream, "seg")));
+    pt_mark(g, 12);
+    LUXB_CUDA(cudaStreamWaitEvent(g->stream, g->ev_join, 0));
+    pt_mark(g, 13);
+    pt_span(g, 14, t_fork, pt_event(g, g->stream));
+  } else {
+    if (g->sb_on) {
+      LUXB_TRY((launch_seg_stream<true, Prog>(g, g->sb_panel, pa, g->sweep.panel_shape, 1, 5, "panel")));
+      pt_mark(g, 1);
+    }
+    if constexpr (kColdHub) {
+      if (g->cs_on) {
+        LUXB_TRY((launch_seg_stream<false, Prog, true>(g, g->sb_cold, ca, g->sweep.cs_shape, g->pull_ctas, 9, "cold-hub")));
+        pt_mark(g, 1);
+      }
+    }
+    LUXB_TRY(wait_cold_exchange(g));
+    LUXB_TRY((launch_seg_kernel<false, Prog>(g, ma, g->sweep.main_shape, g->num_sms, g->pull_ctas, g->stream, "seg")));
+    pt_mark(g, 0);
+  }
+  LUXB_TRY(launch_fixup(g, ma.p, g->sb_main.fix, g->sb_main.d_piece_slot));
+  LUXB_TRY(launch_seg_empties(g, g->sb_main, ma.p, out_buffer));
+  pt_mark(g, 1);
   LUXB_TRY(kt_end(g));
   if (g->sb_on) {
-    CombineArgs<Prog> ca{};
-    ca.hub_vtx = g->d_hub_vtx;
-    ca.n_hub = g->sb_n_hub;
-    ca.n_blocks = g->sb_n_blocks;
-    ca.n_groups = g->sb_n_groups;
-    ca.row_left = g->row_left;
-    ca.sg = g->sb_groups;
-    ca.slot_bits = g->d_slot_bits;
-    ca.slot_pre = g->d_slot_pre;
-    ca.partial = reinterpret_cast<const Acc*>(g->d_sb_partial);
-    ca.x_nat = x_nat;
-    ca.out = out_local;
-    ca.prm = prm;
-    combine_hub_kernel<Prog><<<grid_for(g->sb_n_hub, 256, g->num_sms * 8), 256, 0, g->stream>>>(ca);
+    CombineArgs<Prog> cb{};
+    cb.hub_vtx = g->d_hub_vtx;
+    cb.n_hub = g->sb_n_hub;
+    cb.n_blocks = g->sb_n_blocks;
+    cb.n_groups = g->sb_n_groups;
+    cb.row_left = g->row_left;
+    cb.sg = g->sb_groups;
+    cb.slot_bits = g->d_slot_bits;
+    cb.slot_pre = g->d_slot_pre;
+    cb.partial = reinterpret_cast<const Acc*>(g->d_sb_partial);
+    cb.x_nat = x_nat;
+    cb.out = out_local;
+    cb.prm = prm;
+    combine_hub_kernel<Prog><<<grid_for(g->sb_n_hub, 256, g->num_sms * 8), 256, 0, g->stream>>>(cb);
     LUXB_CUDA(cudaGetLastError());
     g->stats.kernel_launches++;
     pt_mark(g, 6);
@@ -2501,6 +2615,7 @@ static int finish_timed(luxb_graph* g) {
   if (g->pt.per_call) {  // LUXB_PHASE_TIMING=2: one line per luxb_iterate call instead of one per handle
     pt_print(g);
     for (double& v : g->pt.sum) v = 0;
+    g->pt.chain = 0;
     g->pt.cnt = 0;
   }
   LUXB_CUDA(cudaEventRecord(g->ev_end, g->stream));
@@ -3750,6 +3865,9 @@ void luxb_close(luxb_graph* g) {
   if (g->ev_pack) cudaEventDestroy(g->ev_pack);
   if (g->ev_cold) cudaEventDestroy(g->ev_cold);
   if (g->stream2) cudaStreamDestroy(g->stream2);
+  if (g->ev_fork) cudaEventDestroy(g->ev_fork);
+  if (g->ev_join) cudaEventDestroy(g->ev_join);
+  if (g->stream_b) cudaStreamDestroy(g->stream_b);  // idle: it joins the compute stream at the end of every sweep
   for (size_t i = g->owned.size(); i-- > 0;) free_owned(g->owned[i]);  // newest first
   for (cudaEvent_t e : g->kt_events) cudaEventDestroy(e);
   if (g->ev_begin) cudaEventDestroy(g->ev_begin);

@@ -66,14 +66,23 @@ struct SweepSettings {
   double hot_mb = 24.0;        // LUXB_HOT_MB: the hot set
   bool l2_persist = true;      // LUXB_L2_PERSIST=0: no persisting L2 window
   double l2_window_mb = -1.0;  // LUXB_L2_WINDOW_MB: cap on that window (< 0: unset)
+  // LUXB_PANEL_SMS: one rank with the split: the panel kernel runs on this many SMs while the cold-hub and main
+  // kernels run beside it on the others (api.cu: sweep_seg); 0, or >= the SM count: one after another
+  int panel_sms = 40;
 };
 
-// dev aid: LUXB_PHASE_TIMING=1 prints the mean device time of each phase of a PageRank iteration at luxb_close
+// dev aid: LUXB_PHASE_TIMING=1 prints the mean device time of each phase of a PageRank iteration at luxb_close.
+// ev / tag: marks on the compute stream, each timing the phase since the previous mark; span_ev / spans: phases
+// between two events of any stream (the concurrent sweep's side stream, its overlapped region)
 struct PhaseTimer {
+  struct Span { int begin, end, tag; };
   bool on = false, per_call = false;
   std::vector<cudaEvent_t> ev;
   std::vector<int> tag;
-  double sum[12] = {0};
+  std::vector<cudaEvent_t> span_ev;
+  std::vector<Span> spans;
+  double sum[15] = {0};
+  double chain = 0;  // the compute stream's marks summed: the device time of the iterations
   long cnt = 0;
 };
 
@@ -302,6 +311,10 @@ struct luxb_graph {
   bool cold_z = false;             // one rank: d_hot = Z = [hot copies | cold-active values in id order], d_hot_order covers both
   bool cs_on = false;
   PullLayout sb_cold;
+  // concurrent split sweep (one rank, sb_on): the cold-hub and main kernels on stream_b beside the panel kernel on
+  // `stream`; ev_fork / ev_join hand the sweep over and back
+  cudaStream_t stream_b = nullptr;
+  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
 
   // launch configuration resolved once at open time (no getenv / function-static state on the hot path)
   int pull_ctas = 3;

@@ -1,7 +1,9 @@
 // Dev microbenchmark: what random 4-byte gather rate can an H100 sustain, by mechanism and index distribution?
 // build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o /tmp/ubench_gather scripts/ubench_gather.cu
+// run:   /tmp/ubench_gather [scale]   or   /tmp/ubench_gather 27 sms  (L2-resident gathers confined to S SMs, DESIGN §5)
 #include <cstdio>
 #include <cstdlib>
+#include <cstring>
 #include <vector>
 #include "../lux_b200/csrc/build.cuh"
 using namespace luxb;
@@ -59,6 +61,30 @@ __global__ void gather_cpasync(const uint32_t* __restrict__ idx, const float* __
   if (acc == 123.456f) out[0] = acc;
 }
 
+// random gathers confined to the SMs with %smid < s_max: CTAs placed elsewhere leave at once, the others claim chunks of
+// 2048 gathers from a counter.  Does the gather rate scale with SMs, or is it a limit of the whole device?
+__global__ void gather_on_sms(const uint32_t* __restrict__ idx, const float* __restrict__ x, uint64_t m, float* out, uint32_t s_max,
+                              unsigned long long* next) {
+  uint32_t smid;
+  asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+  if (smid >= s_max) return;
+  __shared__ unsigned long long base;
+  float acc = 0.f;
+  for (;;) {
+    __syncthreads();
+    if (threadIdx.x == 0) base = atomicAdd(next, 2048ull);
+    __syncthreads();
+    const uint64_t b = base;
+    if (b >= m) break;
+    float v[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) { const uint64_t i = b + k * 256 + threadIdx.x; v[k] = i < m ? __ldg(x + __ldg(idx + i)) : 0.f; }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc += v[k];
+  }
+  if (acc == 123.456f) out[0] = acc;
+}
+
 template <class F>
 float timeit(F f, int reps = 3) {
   cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
@@ -76,6 +102,17 @@ int main(int argc, char** argv) {
   cudaMalloc(&x, (size_t)n * 4); cudaMalloc(&idx, m * 4); cudaMalloc(&out, 4);
   cudaMemset(x, 0, (size_t)n * 4);
   int sms; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+  if (argc > 2 && !strcmp(argv[2], "sms")) {  // ubench_gather 27 sms: uniform gathers into 24 MB (L2-resident) on S SMs
+    const uint32_t n24 = 6u << 20;
+    unsigned long long* next; cudaMalloc(&next, 8);
+    gen_idx<<<sms * 16, 256>>>(idx, m, 0, scale, n24);
+    cudaDeviceSynchronize();
+    for (int s : {sms, sms - 16, sms - 32, sms - 48, 40, 32}) {
+      float ms = timeit([&] { cudaMemsetAsync(next, 0, 8); gather_on_sms<<<sms * 8, 256>>>(idx, x, m, out, s, next); });
+      printf("  24 MB array, uniform, 8 gathers in flight per thread, %3d SMs: %7.3f ms  %6.1f Ggather/s\n", s, ms, m / ms / 1e6);
+    }
+    return 0;
+  }
   for (int mode = 0; mode < 2; ++mode) {
     gen_idx<<<sms * 16, 256>>>(idx, m, mode, scale, n);
     cudaDeviceSynchronize();
