@@ -84,6 +84,11 @@ typedef enum {
  *    Parallel edges count with their multiplicity; a self-loop never matches;
  *  - delta[v] = sigma[v] * sum of t[w] over the out-edges (v, w) with lev[w] = lev[v] + 1, t[w] = (1 + delta[w]) / sigma[w];
  *  - unreachable vertices have sigma = delta = 0.
+ * sigma counts paths, so it is exact while it is below 2^53: every order of the sum gives the same integer.  Past that,
+ * each sigma is the fp64 sum in the kernels' fixed order (lanes over the edge list, a fixed shuffle tree, 4096-edge
+ * segments added in order): one rank is bitwise reproducible, and sigma equals the in-order sum wherever no sum has more
+ * than two non-zero terms.  A count of 2^1024 or more overflows to inf, and delta and the scores of that source are then
+ * not finite; no error is reported.
  * For a list of sources S: BC[v] = sum over s in S, s != v, of delta_s(v), in fp64, not normalised; a source listed twice
  * counts twice.  S = all vertices gives exact directed BC, a sample the usual estimate; on a graph stored with both
  * directions of every edge the scores are twice the undirected BC.
@@ -106,6 +111,7 @@ typedef enum {
  *    with their multiplicity, but only those at the minimal weight are tight; a self-loop is never tight;
  *  - delta[v] = sigma[v] * sum of t[x] over the tight out-edges (v, x), t[x] = (1 + delta[x]) / sigma[x];
  *  - unreachable vertices have sigma = delta = 0.
+ * sigma is exact below 2^53 and overflows to inf at 2^1024 as for LUXB_BC.
  * Scores accumulate as for LUXB_BC (sum over s in S, s != v, fp64, not normalised, repeats count).  Unit weights give
  * LUXB_BC exactly: D = lev, and sigma, delta and the scores are bit for bit equal.  luxb_bc_source_state returns D as
  * `lev`.  Values, luxb_iterate / luxb_run_to_convergence / luxb_check, luxb_stats and the phase timing behave as for
